@@ -1,15 +1,17 @@
 #!/usr/bin/env python
-"""bench.py — J/K Fock-build seconds per SCF iteration (BASELINE.json metric) on B200.
+"""bench.py — J/K Fock-build seconds per SCF iteration (BASELINE.json metric) on H100.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--no-df]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--no-df] [--dump-outputs DIR]
 
 A "step" = one J/K Fock build (one get_jk-equivalent call) for the workload's density matrix.
 Headline workload (the top-level value / e2e / roofline of the JSON line): configs[1] of BASELINE.json, benzene / cc-pVTZ RHF,
 4-center direct J/K.  The SAME JSON line carries, under "df", one full record (value, e2e, roofline with per-stage figures,
 parity) for every density-fitting configuration of BASELINE.json that fits the N GPUs of the run:
     c60-def2svp-df            configs[2]  (N >= 1)
-    taxol-def2tzvp-df         configs[3]  (N >= 1: the 111 GB tensor fits one 180 GB B200; sharded by auxiliary rows for N > 1)
-    gly30-ccpvdz-df-wb97x     configs[4]  (N >= 4: omega-B97X needs get_jk on the Coulomb tensor AND get_k(omega=0.3) on a second,
+    taxol-def2svp-df                      (N >= 1: the 28 GB tensor fits one H100, the int8 slices of all its rows do not:
+                                           resident and per-step re-cut slices both run)
+    taxol-def2tzvp-df         configs[3]  (N >= 2: the 111 GB tensor is sharded by auxiliary rows over 80 GB H100s)
+    gly30-ccpvdz-df-wb97x     configs[4]  (N >= 8: omega-B97X needs get_jk on the Coulomb tensor AND get_k(omega=0.3) on a second,
                                            erf-attenuated tensor, 2 x 196.6 GB)
 Each DF record is measured by a child process per rank (own NCCL group on another port), so that a failure or a hang in one
 configuration cannot take the headline number down with it; a per-record timeout bounds the whole run.
@@ -22,13 +24,17 @@ Timed numbers (headline and every DF record)
   e2e                 : the same build through the public plugin call (VHFOpt.get_jk / DF.get_jk / ShardedJK.get_jk) with pinned
                         HOST buffers (H2D of D, C_occ and D2H of J,K inside the timed region).
   roofline            : direct: all class launches of one build against the measured FP64 FMA-pipe peak (b200jk_fp64_peak).
-                        DF: the dominant kernel (stage 1 of DF-K, tcgen05 int8 slices) per launch from CUDA events the library
-                        records around every launch, against 2 x the measured bf16 tensor peak; other stages listed beside it.
+                        DF: the dominant kernel (stage 1 of DF-K, int8 slices on wgmma) per launch from CUDA events the library
+                        records around every launch, against the int8 tensor peak (2 x bf16); other stages listed beside it.
   parity              : max |dJ|, |dK| of the (all-reduced) result against oracle-made golden vectors (tests/golden) on the
                         reference's own parity density (seed 1), at every N.
   cpu_baseline        : rank 0, N = 1 only.
+--steps K sets the timed steps of the headline AND of every DF record.
+--dump-outputs DIR writes what the timed path returned in its last timed step (J, K and, for omega-B97X, K of the
+attenuated tensor) as float64 DIR/<name>.npy; DF records prefix the workload name.  Arrays over 8 MB are replaced by a
+fixed sample of 2^20 elements (seeded, the same for the same shape), so that two builds can be compared output for output.
 --impl reference times the CPU arm alone with the same JSON schema: the reference's own driver/screening/digestion C
-(oracle/_ref, compiled from /root/reference/pyscf/lib/vhf) around the oracle's integral function; every step is a bounded
+(oracle/_ref, compiled from the reference's pyscf/lib/vhf) around the oracle's integral function; every step is a bounded
 sample (every m-th surviving shell quartet per thread, time x m).
 """
 import argparse
@@ -53,12 +59,13 @@ WORKLOADS = {
     'gly30-ccpvdz-df': dict(geom='gly30', basis='cc-pvdz', nocc=455, kind='df'),               # full-range part of configs[4]
     'gly30-ccpvdz-df-wb97x': dict(geom='gly30', basis='cc-pvdz', nocc=455, kind='df', omega=0.3),   # BASELINE configs[4]
     'taxol-def2tzvp-df': dict(geom='taxol', basis='def2-tzvp', nocc=226, kind='df'),           # BASELINE configs[3]
+    'taxol-def2svp-df': dict(geom='taxol', basis='def2-svp', nocc=226, kind='df'),
     'gly4-ccpvdz-df': dict(geom='gly4', basis='cc-pvdz', nocc=65, kind='df'),
     'gly4-ccpvdz-df-wb97x': dict(geom='gly4', basis='cc-pvdz', nocc=65, kind='df', omega=0.3),
 }
-# DF records appended to the headline line: (workload, smallest N it fits, steps, warmup, child timeout in seconds)
-DF_EXTRAS = [('c60-def2svp-df', 1, 10, 3, 240), ('taxol-def2tzvp-df', 1, 4, 3, 300), ('gly30-ccpvdz-df-wb97x', 4, 4, 3, 300)]
-TENSOR_GB = {'taxol-def2tzvp-df': 111.2, 'gly30-ccpvdz-df-wb97x': 2 * 196.6, 'c60-def2svp-df': 12.7}
+# DF records appended to the headline line: (workload, smallest N whose 80 GB H100s hold its tensors, child timeout in seconds)
+DF_EXTRAS = [('c60-def2svp-df', 1, 240), ('taxol-def2svp-df', 1, 300), ('taxol-def2tzvp-df', 2, 300), ('gly30-ccpvdz-df-wb97x', 8, 300)]
+TENSOR_GB = {'taxol-def2tzvp-df': 111.2, 'gly30-ccpvdz-df-wb97x': 2 * 196.6, 'c60-def2svp-df': 12.7, 'taxol-def2svp-df': 28.3}
 
 
 def scf_like_dm(nao, nocc, seed=1):
@@ -147,21 +154,19 @@ def algorithmic_bytes(opt):
     return 3 * n * n * 8 + st['n_pairs'] * 48
 
 
-def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch of `kernel` from the committed `ncu --set full` summary of the
-    C60 bench command (profiles/r02_ncu_summary.txt); None when the profile is not there."""
-    try:
-        tot, on = 0.0, False
-        for line in open(os.path.join(ROOT, 'profiles', 'r02_ncu_summary.txt')):
-            if line.startswith('kernel:'):
-                on = kernel in line
-            elif on and ('dram__bytes_read.sum' in line or 'dram__bytes_write.sum' in line):
-                f = line.split()
-                scale = {'byte': 1.0, 'Kbyte': 1e3, 'Mbyte': 1e6, 'Gbyte': 1e9, 'Tbyte': 1e12}.get(f[2] if len(f) > 2 else 'byte', 1.0)
-                tot += float(f[1]) * scale
-        return tot or None
-    except Exception:
-        return None
+DUMP_SAMPLE_BYTES = 8 << 20
+
+
+def dump_outputs(d, prefix, arrays):
+    """Write {name: array} as float64 d/<prefix><name>.npy; an array over DUMP_SAMPLE_BYTES becomes a fixed seeded sample of
+    2^20 of its elements (the same indices for the same shape)."""
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a, dtype=np.float64)
+        if a.nbytes > DUMP_SAMPLE_BYTES:
+            idx = np.sort(np.random.RandomState(0).choice(a.size, 1 << 20, replace=False))
+            a = a.ravel()[idx]
+        np.save(os.path.join(d, prefix + name + '.npy'), a)
 
 
 def load_peaks():
@@ -197,14 +202,14 @@ def golden_parity(workload, vj, vk, what):
             'against': 'tests/golden/%s (full J/K of the CPU oracle)' % name, 'bar': 1e-9}
 
 
-SIZE_FIXTURE = {'c60-def2svp-df': ('c60', None), 'taxol-def2tzvp-df': ('taxol', None), 'gly30-ccpvdz-df': ('gly30', None),
+SIZE_FIXTURE = {'c60-def2svp-df': ('c60', None), 'taxol-def2tzvp-df': ('taxol', None), 'taxol-def2svp-df': ('taxol_svp', None), 'gly30-ccpvdz-df': ('gly30', None),
                 'gly30-ccpvdz-df-wb97x': ('gly30', 'gly30_lr'), 'gly4-ccpvdz-df': ('gly4', None), 'gly4-ccpvdz-df-wb97x': ('gly4', None)}
 
 
 def df_size_parity(workload, eng, eng2, step_device, out_d, res_dev, dev, rank, world, dist):
     """Oracle parity of a DF configuration AT ITS SIZE, at every N (fixtures: tools/make_golden_df_size.py, tests/golden/df_size_*):
     sampled tensor columns over the auxiliary rows of every rank, and J/K of the fixture's slab density through BOTH K engines
-    (orbital-tagged: tcgen05 occupied-orbital algorithm; bare matrix: general-density algorithm), all-reduced like a timed step."""
+    (orbital-tagged: occupied-orbital algorithm; bare matrix: general-density algorithm), all-reduced like a timed step."""
     import torch
     sys.path.insert(0, os.path.join(ROOT, 'tests'))
     import df_size_check as S
@@ -343,6 +348,9 @@ def measure(args, rank, world, dist):
     step_ms = [a.elapsed_time(b) for a, b in evs]
     ms_per_step = float(np.mean(step_ms))
     res_dev = out_d.cpu().numpy().copy()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, (args.workload + '_') if args.child else '',
+                     dict(zip(('vj', 'vk', 'vk_lr'), res_dev)))
     # ---- parity on the reference's own test density (seed 1, D + D^T; general-density path for DF) against the oracle golden
     par = None
     try:
@@ -408,7 +416,7 @@ def measure(args, rank, world, dist):
         return None
     # ---- roofline
     peaks = load_peaks()
-    hbm_peak = peaks.get('hbm_gbs', 6650.0)
+    hbm_peak = peaks.get('hbm_gbs', 3350.0)
     if not is_df:
         from pyscf_b200.flops import direct_jk_flops
         peak = ctypes.c_double(0)
@@ -423,7 +431,7 @@ def measure(args, rank, world, dist):
                 'peak_source': 'b200jk_fp64_peak DFMA micro-benchmark (MEASURED_PEAKS.json has no fp64 entry)',
                 'hbm': {'bound': 'hbm', 'achieved': bytes_alg / (kernel_ms * 1e-3) / 1e9, 'peak': hbm_peak, 'unit': 'GB/s',
                         'frac': bytes_alg / (kernel_ms * 1e-3) / 1e9 / hbm_peak, 'alg_bytes_per_step': bytes_alg,
-                        'peak_source': 'MEASURED_PEAKS.json hbm_gbs (of measured)' if peaks else 'fallback 6650'}}
+                        'peak_source': 'MEASURED_PEAKS.json hbm_gbs (of measured)' if peaks else 'H100 SXM data sheet, 3350 GB/s'}}
         path = '4-center direct J/K (hermi=1, with_j, with_k)'
     else:
         naux = eng.get_naoaux()
@@ -432,7 +440,7 @@ def measure(args, rank, world, dist):
         naux2 = eng2.get_naoaux() if eng2 is not None else 0         # rows of the erf-attenuated tensor (fewer: eigenvalue cut of its metric)
         fp64_flops = 4.0 * (naux + naux2) * nao * nao * w['nocc']    # dsymm + dgemm count of the reference (SURVEY §8d), summed over the K builds
         int8_ops = fp64_flops * nsl
-        bf16_peak = peaks.get('bf16_tflops_sustained', 1400.0)
+        bf16_peak = peaks.get('bf16_tflops_sustained', 989.0)
         tensor_peak = 2 * bf16_peak
         cderi_bytes = naux * nao * (nao + 1) / 2 * 8
 
@@ -447,15 +455,15 @@ def measure(args, rank, world, dist):
         for k in ('k_gemm1', 'k_gemm2'):
             ms_k, n_k = stg[k]
             if n_k:
-                stages[k] = {'kernel': 'i8gemm_ar_kernel (stage 1: Y = A C~)' if k == 'k_gemm1' else 'i8gemm_ar_kernel (stage 2: K += Y Y^T, accumulate mode)', 'bound': 'tensor',
+                stages[k] = {'kernel': 'i8gemm_kernel (stage 1: Y = A C~)' if k == 'k_gemm1' else 'i8gemm_kernel (stage 2: K += Y Y^T, accumulate mode)', 'bound': 'tensor',
                              'launches_per_step': n_k, 'ms_per_launch': ms_k / n_k, 'ms_per_step': ms_k,
                              'alg_int8_ops_per_launch': half_ops / n_k, 'achieved': half_ops / (ms_k * 1e-3) / 1e12,
                              'peak': tensor_peak, 'unit': 'TOP/s (int8)', 'frac': half_ops / (ms_k * 1e-3) / 1e12 / tensor_peak}
                 if k == 'k_gemm2':
-                    # the kernel computes only the 128 x 64 tiles that touch the upper triangle of the symmetric product
-                    mt_, nt_ = (nao + 127) // 128, (nao + 63) // 64
-                    done = sum(max(0, nt_ - 2 * a) for a in range(mt_))
-                    fexec = done * 128.0 * 64.0 / (nao * nao)
+                    # the kernel computes only the 128 x 32 tiles that touch the upper triangle of the symmetric product
+                    mt_, nt_ = (nao + 127) // 128, (nao + 31) // 32
+                    done = sum(max(0, nt_ - 4 * a) for a in range(mt_))
+                    fexec = done * 128.0 * 32.0 / (nao * nao)
                     stages[k].update({'executed_frac_of_alg_ops': fexec, 'achieved_executed': stages[k]['achieved'] * fexec,
                                       'frac_executed': stages[k]['frac'] * fexec,
                                       'note': 'algorithmic count = the full Y Y^T product of the reference dgemm (SURVEY 8d); the kernel executes '
@@ -475,8 +483,8 @@ def measure(args, rank, world, dist):
         g1 = stages.get('k_gemm1')
         if g1:     # the dominant kernel: stage 1 of DF-K
             roof = {'bound': 'tensor', 'achieved': g1['achieved'], 'peak': tensor_peak, 'unit': 'TOP/s (int8)', 'frac': g1['frac'],
-                    'traffic': ncu_traffic('i8gemm_ar_kernel') if args.workload == 'c60-def2svp-df' and world == 1 else None,
-                    'kernel': 'i8gemm_ar_kernel (tcgen05.mma.kind::i8, stage 1 of DF-K: Y = (P|mu nu) C~), CUDA events around '
+                    'traffic': None,
+                    'kernel': 'i8gemm_kernel (wgmma s8, stage 1 of DF-K: Y = (P|mu nu) C~), CUDA events around '
                               'each of its launches inside the timed steps',
                     'ms_per_launch': g1['ms_per_launch'], 'launches_per_step': g1['launches_per_step'],
                     'alg_int8_ops_per_launch': g1['alg_int8_ops_per_launch']}
@@ -489,10 +497,10 @@ def measure(args, rank, world, dist):
                                 'note': 'all int8 slice-GEMM work over the whole DF J+K build time (J passes, slicing, both GEMM stages)',
                                 'fp64_equiv_flops_per_step': fp64_flops,
                                 'fp64_equiv_tflops': fp64_flops / world / (kernel_ms * 1e-3) / 1e12},
-                'peak_source': 'tensor: 2 x MEASURED_PEAKS.json bf16_tflops_sustained (int8 dense = 2x bf16 on sm_100a; sustained '
+                'peak_source': 'tensor: 2 x MEASURED_PEAKS.json bf16_tflops_sustained (int8 dense = 2x bf16 on sm_90a; sustained '
                                'because the kernel runs inside a long step); hbm: MEASURED_PEAKS.json hbm_gbs'
-                               if peaks else 'fallback 2 x 1400 TFLOP/s, 6650 GB/s (B200_PROFILING.md)'})
-        path = 'DF J/K (cderi resident, K via tcgen05 int8 slices, %d slices)' % ns
+                               if peaks else 'H100 SXM data sheet: 2 x 989 TFLOP/s (int8 dense), 3350 GB/s'})
+        path = 'DF J/K (cderi resident, K via int8 slices on the tensor cores, %d slices)' % ns
         if omega2:
             path += ' + get_k(omega=%g) on the erf-attenuated tensor (omega-B97X, pyscf/dft/rks.py:123-127)' % omega2
     # ---- CPU baseline (oracle port), rank 0, N=1 only
@@ -559,7 +567,7 @@ def child_env(rank, world, port):
     return env
 
 
-def run_extra(name, steps, warmup, timeout, rank, world, base_port, idx, no_cpu):
+def run_extra(name, steps, warmup, timeout, rank, world, base_port, idx, no_cpu, dump):
     """Run one DF record in a child process of this rank; rank 0 returns the record (or an error record)."""
     tag = '%d_%d' % (base_port, idx)
     outp = '/tmp/b200jk_bench_%s.json' % tag
@@ -575,6 +583,8 @@ def run_extra(name, steps, warmup, timeout, rank, world, base_port, idx, no_cpu)
            '--gpus', str(world), '--out', outp]
     if no_cpu:
         cmd.append('--no-cpu')
+    if dump:
+        cmd += ['--dump-outputs', os.path.abspath(dump)]
     t0 = time.time()
     log = open('/tmp/b200jk_bench_%s_r%d.log' % (tag, rank), 'w')
     proc = subprocess.Popen(cmd, env=child_env(rank, world, port), stdout=log, stderr=subprocess.STDOUT)
@@ -643,10 +653,10 @@ def run_ours(args, rank, world):
         base_port = int(os.environ.get('MASTER_PORT', '29500'))
         df = {}
         t_start = time.time()
-        for idx, (name, nmin, steps, warmup, timeout) in enumerate(DF_EXTRAS):
+        for idx, (name, nmin, timeout) in enumerate(DF_EXTRAS):
             if world < nmin:
                 if rank == 0:
-                    df[name] = {'skipped': 'needs >= %d GPUs: %.1f GB of tensors (+ workspaces) against 180 GB of HBM per B200'
+                    df[name] = {'skipped': 'needs >= %d GPUs: %.1f GB of tensors (+ workspaces) against 80 GB of HBM per H100'
                                            % (nmin, TENSOR_GB[name])}
                 continue
             left = args.df_budget - (time.time() - t_start)
@@ -658,7 +668,8 @@ def run_ours(args, rank, world):
                 if rank == 0:
                     df[name] = {'skipped': 'time budget of the bench run exhausted (--df-budget %d s)' % args.df_budget}
                 continue
-            rec = run_extra(name, steps, warmup, min(timeout, left), rank, world, base_port, idx, args.no_cpu)
+            rec = run_extra(name, args.steps, args.warmup, min(timeout, left), rank, world, base_port, idx, args.no_cpu,
+                            args.dump_outputs)
             if world > 1:
                 dist.barrier()
             if rank == 0:
@@ -824,6 +835,8 @@ def main():
     ap.add_argument('--no-df', action='store_true', help='headline workload only (no "df" records)')
     ap.add_argument('--df-budget', type=int, default=560, help='seconds the DF records of one run may take in total')
     ap.add_argument('--ref-stride', type=int, default=8, help='--impl reference: evaluate every m-th surviving shell quartet per step')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write the J/K of the last timed step (and of every DF record) as DIR/<name>.npy')
     ap.add_argument('--child', action='store_true', help=argparse.SUPPRESS)
     ap.add_argument('--out', default=None, help=argparse.SUPPRESS)
     args = ap.parse_args()

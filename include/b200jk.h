@@ -1,5 +1,5 @@
 /*
- * b200jk.h — C ABI of libb200jk.so, the B200-native J/K Fock-matrix builder.
+ * b200jk.h — C ABI of libb200jk.so, the H100-native J/K Fock-matrix builder.
  *
  * Every entry point takes plain pointers and sizes (numpy-owned host buffers); the library owns all
  * device memory, streams and NCCL communicators inside the opaque handle.  All functions return 0 on
@@ -96,7 +96,7 @@ int b200jk_df_naux(b200jk_handle h, int* naux);
 /* b200jk_df_jk with dm, occ_coeff, vj, vk already on the handle's device (device pointers, no host copies). */
 int b200jk_df_jk_device(b200jk_handle h, const double* dm_dev, int n_dm, int nao, const double* occ_dev, int nocc, int hermi,
                         double* vj_dev, double* vk_dev);
-/* K-build engine for the occupied-orbital path: mode 1 (default) = tcgen05 int8-slice GEMMs (i8gemm.cuh) with
+/* K-build engine for the occupied-orbital path: mode 1 (default) = int8-slice tensor-core GEMMs (wgmma, i8gemm.cuh) with
  * `nslices` 7-bit slices (7 -> ~1e-11 relative), mode 0 = cuBLAS DGEMM on the FP64 pipe (kept as yardstick). */
 int b200jk_df_set_kmode(b200jk_handle h, int mode, int nslices);
 /* Device time of the stages of the last b200jk_df_jk[_device] call, from CUDA events recorded around every launch on
@@ -104,9 +104,9 @@ int b200jk_df_set_kmode(b200jk_handle h, int mode, int nslices);
  * pyscf/df/df_jk.py:412): ms[s] = summed milliseconds, count[s] = launches of stage s; n <= B200JK_DF_NSTAGE entries. */
 enum { B200JK_DF_STAGE_J_RHO = 0,    /* rho_P = sum cderi[P,:] dmtril           (streams the tensor once) */
        B200JK_DF_STAGE_J_ACC = 1,    /* J~ = sum_P rho_P cderi[P,:]             (streams it a second time) */
-       B200JK_DF_STAGE_K_GEMM1 = 2,  /* Y = (P|mu nu) C~     tcgen05 i8gemm_ar_kernel */
+       B200JK_DF_STAGE_K_GEMM1 = 2,  /* Y = (P|mu nu) C~     i8gemm_kernel (wgmma) */
        B200JK_DF_STAGE_K_SLICE = 3,  /* int8 slicing of Y */
-       B200JK_DF_STAGE_K_GEMM2 = 4,  /* K += Y Y^T           tcgen05 i8gemm_kernel */
+       B200JK_DF_STAGE_K_GEMM2 = 4,  /* K += Y Y^T           i8gemm_kernel (wgmma) */
        B200JK_DF_NSTAGE = 5 };
 int b200jk_df_stage_times(b200jk_handle h, double* ms, int* count, int n);
 /* Rows of the tensor held by this handle: [row0, row0+nrow) of the naux rows.  The whole tensor unless
@@ -148,7 +148,7 @@ int b200jk_fp64_peak(b200jk_handle h, double* tflops);
  * ms[100]: entry [cb*10+ck], pair class id = l1*(l1+1)/2+l2 (ss,ps,pp,ds,dp,dd,fs,fp,fd,ff). */
 int b200jk_set_profile(b200jk_handle h, int on);
 int b200jk_get_class_times(b200jk_handle h, double* ms, int n);
-/* Self-test of the tcgen05 int8-slice GEMM used by DF-K: C[M,N] = A[M,K] B[N,K]^T with `ns` 7-bit slices. */
+/* Self-test of the int8-slice tensor-core GEMM used by DF-K: C[M,N] = A[M,K] B[N,K]^T with `ns` 7-bit slices. */
 int b200jk_i8gemm_test(b200jk_handle h, int M, int N, int K, const double* A, const double* B, double* C, int ns,
                        int symmetric);
 int b200jk_get_stats(b200jk_handle h, b200jk_stats* out);

@@ -29,7 +29,7 @@ extern "C" const char* b200jk_version(void)
 #ifdef B200JK_EMULATE
     return "b200jk 0.1 (CPU SIMT emulation — tests only)";
 #else
-    return "b200jk 0.1 (sm_100a)";
+    return "b200jk 0.1 (sm_90a)";
 #endif
 }
 
@@ -369,8 +369,8 @@ static int direct_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, 
                 for (const ShellPair& sp : K.kept) pk += sp.nprim;
                 double pq = pb * pk * (cb == ck ? 0.5 : 1.0);
                 int nr = (B.la + B.lb + K.la + K.lb) / 2 + 1;
-                // milliseconds on one B200: least-squares fit to the measured class times of benzene/cc-pVTZ
-                // (profiles/r01_class_times_direct.json, mean abs error 20 %): launch/tail + roots + root sum + digestion
+                // relative class cost (launch/tail + roots + root sum + digestion), a least-squares fit to measured class times
+                // of benzene/cc-pVTZ (mean abs error 20 %); only ratios matter: launch order and the multi-GPU balance
                 double cost = 0.0976 + 3.14e-9 * pq * nr + 7.6e-10 * pq * nr * ncomp + 2.38e-9 * nq * ncomp + 1.3e-7 * nq;
                 if (h->have_costs && h->class_cost[cb * NPC + ck] > 0.0) cost = h->class_cost[cb * NPC + ck];   // measured on this machine
                 jobs.push_back({cb, ck, cost});

@@ -61,7 +61,7 @@ struct DFState {
     double *d_dmtril = nullptr, *d_rho = nullptr, *d_vjtril = nullptr, *d_A = nullptr, *d_Y = nullptr, *d_occ = nullptr,
            *d_dm = nullptr, *d_vk = nullptr, *d_vj = nullptr;
     size_t ws_rows = 0, ws_nocc = 0, ws_ndm = 0, ws_occ_ndm = 0;
-    int k_mode = 1;      // 0: cuBLAS DGEMM (FP64 pipe), 1: tcgen05 int8 slices (i8gemm.cuh)
+    int k_mode = 1;      // 0: cuBLAS DGEMM (FP64 pipe), 1: int8 slices on the tensor cores (i8gemm.cuh)
     int k_slices = 7;
     double* d_Y2 = nullptr; double* d_occT = nullptr; size_t y2_cap = 0, occT_cap = 0;
 #ifndef B200JK_EMULATE
@@ -315,7 +315,7 @@ static void rows_dot(const double* M, long nrow, long ncol, const double* x, lon
 static void cols_acc(const double* M, long nrow, long ncol, const double* x, int xstride, double* y, long ystride, int n_dm, cudaStream_t st)
 {
     const unsigned ncb = (unsigned)((ncol + 255) / 256);
-    unsigned gy = (unsigned)std::max<long>(1, std::min<long>(nrow / 64, (6L * 148 * 8 + ncb - 1) / ncb));
+    unsigned gy = (unsigned)std::max<long>(1, std::min<long>(nrow / 64, (6L * device_sm_count() * 8 + ncb - 1) / ncb));
     dfj_acc_kernel<<<dim3(ncb, gy), 256, 0, st>>>(M, x, y, ncol, 0, (int)nrow, xstride, n_dm, ystride);
     CK(cudaGetLastError());
 }
@@ -982,8 +982,8 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
             mark(B200JK_DF_STAGE_J_ACC);
             {
                 const unsigned ncb = (unsigned)((npair + 255) / 256);
-                // >= ~6 waves of 148 x 8 CTAs, each row range >= 64 rows
-                unsigned gy = (unsigned)std::max<long>(1, std::min<long>((r_hi - r_lo) / 64, (6L * 148 * 8 + ncb - 1) / ncb));
+                // >= ~6 waves of 8 CTAs per SM, each row range >= 64 rows
+                unsigned gy = (unsigned)std::max<long>(1, std::min<long>((r_hi - r_lo) / 64, (6L * device_sm_count() * 8 + ncb - 1) / ncb));
                 dfj_acc_kernel<<<dim3(ncb, gy), 256, 0, st>>>(d->d_cderi, d->d_rho, d->d_vjtril, npair, r_lo, r_hi - r_lo, naux, n_dm, npair);
             }
             launches++;
@@ -1109,7 +1109,7 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
 #ifndef B200JK_EMULATE
                     const double one = 1.0, zero = 0.0;
                     if (tc) {
-                        // tcgen05 path: Y2[nu][(P,i)] = sum_mu A_P[nu,mu] Ct[i,mu] ; K += Y2 Y2^T (upper triangle)
+                        // tensor-core path: Y2[nu][(P,i)] = sum_mu A_P[nu,mu] Ct[i,mu] ; K += Y2 Y2^T (upper triangle)
                         if (r0 == r_lo || n_dm > 1) {
                             // right factor of stage 1 as rows [ncol][nao]: C~^T, or D^T for the general-density algorithm
                             TransposeFn tr{use_occ ? d->d_occ + (size_t)s * nao * nocc : d->d_dm + (size_t)s * n2, d->d_occT, nao, ncol};
@@ -1154,9 +1154,7 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
                         tick(2);
                         mark(B200JK_DF_STAGE_K_GEMM2);
                         // K += Y Y^T (orbitals) or Y G^T (general density; only its upper triangle when D, hence K, is symmetric)
-                        static const bool old_g2 = getenv("B200JK_G2_OLD") != nullptr;   // yardstick: the round-1 stage-2 kernel
-                        if (old_g2) i8g::gemm(d->SY, use_occ ? d->SY : d->SG, d->d_vk + (size_t)s * n2, nao, 0, k_sym, st);
-                        else i8g::gemm_ar_acc(d->SY, use_occ ? d->SY : d->SG, d->d_vk + (size_t)s * n2, nao, k_sym, st);
+                        i8g::gemm_ar_acc(d->SY, use_occ ? d->SY : d->SG, d->d_vk + (size_t)s * n2, nao, k_sym, st);
                         mark(-1);
                         tick(3);
                         if (prof && r0 + kb >= r_hi) {

@@ -1,4 +1,4 @@
-// i8gemm.cu — host side of the tcgen05 int8-slice GEMM (see i8gemm.cuh) + a C-ABI self-test entry.
+// i8gemm.cu — host side of the int8-slice tensor-core GEMM (see i8gemm.cuh) + a C-ABI self-test entry.
 #include "host_common.hpp"
 #ifndef B200JK_EMULATE
 #include <cudaTypedefs.h>
@@ -164,95 +164,84 @@ void split_packed(SliceStack& S, const double* cderi, long npair, int nao, int n
     split_packed_into(S, 0, cderi, npair, nao, nr, rowexp, st);
 }
 
-// stage-1 GEMM of DF-K with all slice-pair groups resident in TMEM (i8gemm_ar_kernel): rows [a_row0, a_row0+M) of A
+static int sm_count()
+{
+    static int nsm = 0;
+    if (!nsm) {
+        int dev = 0;
+        CK(cudaGetDevice(&dev));
+        CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
+    }
+    return nsm;
+}
+
+template <int NS>
+static void launch_ns(unsigned grid, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& P, cudaStream_t st)
+{
+    static bool configured = false;
+    if (!configured) {
+        CK(cudaFuncSetAttribute(i8gemm_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(NS)));
+        configured = true;
+    }
+    i8gemm_kernel<NS><<<grid, NTHREADS, smem_bytes(NS), st>>>(ta, tb, P);
+}
+// the slice count is a template parameter of the kernel: the accumulators of all slice-pair groups live in registers
+static void launch(unsigned grid, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& P, cudaStream_t st)
+{
+    switch (P.ns) {
+    case 1: launch_ns<1>(grid, ta, tb, P, st); break;
+    case 2: launch_ns<2>(grid, ta, tb, P, st); break;
+    case 3: launch_ns<3>(grid, ta, tb, P, st); break;
+    case 4: launch_ns<4>(grid, ta, tb, P, st); break;
+    case 5: launch_ns<5>(grid, ta, tb, P, st); break;
+    case 6: launch_ns<6>(grid, ta, tb, P, st); break;
+    case 7: launch_ns<7>(grid, ta, tb, P, st); break;
+    case 8: launch_ns<8>(grid, ta, tb, P, st); break;
+    default: throw std::runtime_error("i8gemm: slice count out of range");
+    }
+    CK(cudaGetLastError());
+}
+
+// stage-1 GEMM of DF-K: rows [a_row0, a_row0+M) of A times B^T, one work item per tile, persistent grid
 void gemm_ar(const SliceStack& A, int a_row0, int M, const SliceStack& B, double* C, long ldc, int inner, cudaStream_t st,
              unsigned long long* rowmax, const SliceStack* Yout, int y_ncolp)
 {
     if (A.Kp != B.Kp || A.ns != B.ns) throw std::runtime_error("i8gemm_ar: operand stacks disagree");
-    if (A.ns * AR_BN > 512) throw std::runtime_error("i8gemm_ar: too many slices for TMEM");
-    static bool configured = false;
-    static int nsm = 148;
-    if (!configured) {
-        CK(cudaFuncSetAttribute(i8gemm_ar_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AR_SMEM_MAX));
-        int dev = 0;
-        CK(cudaGetDevice(&dev));
-        CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-        configured = true;
-    }
-    static const int nsa_env = getenv("B200JK_AR_NSA") ? atoi(getenv("B200JK_AR_NSA")) : 0;   // tuning: A ring depth
-    int nsa = AR_MAXA;
-    while (nsa > 2 && ar_smem_bytes(nsa, A.ns) > AR_SMEM_MAX) nsa--;
-    if (nsa_env >= 2 && nsa_env < nsa) nsa = nsa_env;
+    if (A.ns < 1 || A.ns > MAXS) throw std::runtime_error("i8gemm_ar: slice count out of range");
+    const int nsm = sm_count();
     CUtensorMap ta, tb;
     make_tmap(&ta, A.q, (uint64_t)A.ns * A.Rp, A.Kp, BM);
-    make_tmap(&tb, B.q, (uint64_t)B.ns * B.Rp, B.Kp, AR_BN);
+    make_tmap(&tb, B.q, (uint64_t)B.ns * B.Rp, B.Kp, BN);
     GemmParams P{};
     P.M = M; P.N = B.R; P.Kp = A.Kp; P.Mp = A.Rp; P.Np = B.Rp; P.ns = A.ns; P.symmetric = 0;
-    P.Ea = A.E; P.Eb = B.E; P.C = C; P.ldc = ldc; P.inner = inner; P.a_row0 = a_row0; P.ksplit = 1; P.dbg = nullptr;
-    static const int stack = getenv("B200JK_AR_STACK") ? atoi(getenv("B200JK_AR_STACK")) : 1;   // 0: one slice pair per MMA (tuning yardstick)
-    P.stack = stack;
-    P.nsa = nsa;
-    const int ntiles = ((B.R + AR_BN - 1) / AR_BN) * ((M + BM - 1) / BM);
-    P.ar_ntiles = ntiles; P.ar_ksplit = 1; P.ar_kb_per = A.Kp / BK; P.accumulate = 0; P.rowmax = rowmax;
+    P.Ea = A.E; P.Eb = B.E; P.C = C; P.ldc = ldc; P.inner = inner; P.a_row0 = a_row0;
+    const int ntiles = ((B.R + BN - 1) / BN) * ((M + BM - 1) / BM);
+    P.ntiles = ntiles; P.ksplit = 1; P.kb_per = A.Kp / BK; P.accumulate = 0; P.rowmax = rowmax;
     if (Yout) {
         if (inner <= 0 || (y_ncolp & 15) || y_ncolp < B.R || (long)((M + inner - 1) / inner) * y_ncolp > Yout->Kp || Yout->R != inner)
             throw std::runtime_error("i8gemm_ar: inconsistent Y stack");
         P.yq = Yout->q; P.Ey = Yout->E; P.y_Rp = Yout->Rp; P.y_Kp = Yout->Kp; P.y_ncolp = y_ncolp;
     }
-    static const int persist = getenv("B200JK_AR_PERSIST") ? atoi(getenv("B200JK_AR_PERSIST")) : 1;   // 0: one tile per CTA (yardstick)
-    dim3 grid(persist ? std::min(ntiles, nsm) : ntiles);
-    static const bool dbg = getenv("B200JK_I8_DEBUG") != nullptr;   // cycle stamps of CTA 0 (tuning)
-    static long long* d_dbg = nullptr;
-    static int dbg_left = 2;
-    if (dbg && dbg_left > 0) {
-        if (!d_dbg) d_dbg = (long long*)dev_alloc(64 * 8);
-        dev_zero(d_dbg, 64 * 8, st);
-        P.dbg = d_dbg;
-    }
-    i8gemm_ar_kernel<<<grid, NTHREADS, ar_smem_bytes(nsa, A.ns), st>>>(ta, tb, P);
-    if (P.dbg) {
-        long long hd[64];
-        d2h(hd, d_dbg, 64 * 8, st);
-        CK(cudaStreamSynchronize(st));
-        dbg_left--;
-        for (int it = 0; it < 6; it++)
-            fprintf(stderr, "[i8gemm_ar CTA0 tile %d] mma: wait_tmem %lld issue %lld | epi: wait_acc %lld drain %lld store %lld | tile period %lld cycles\n", it,
-                    hd[it * 8 + 1] - hd[it * 8 + 0], hd[it * 8 + 2] - hd[it * 8 + 1], hd[it * 8 + 4] - hd[it * 8 + 3],
-                    hd[it * 8 + 5] - hd[it * 8 + 4], hd[it * 8 + 6] - hd[it * 8 + 5], it ? hd[it * 8 + 6] - hd[(it - 1) * 8 + 6] : 0LL);
-    }
-    CK(cudaGetLastError());
+    launch((unsigned)std::min(ntiles, nsm), ta, tb, P, st);
 }
 
-// C += A B^T (upper triangle only when symmetric) on the A-stationary kernel with all slice-pair groups resident in TMEM
-// (i8gemm_ar_kernel): stage 2 of DF-K.  Against i8gemm_kernel's one (A_k, B_l) tile pair per pipeline stage this loads every
-// A slice tile once per K block and multiplies it with all its B slices: half the operand traffic per output column.
-// Work items = tiles x K ranges, sized to fill whole waves of the persistent grid.
+// C += A B^T (upper triangle only when symmetric): stage 2 of DF-K.  Work items = tiles x K ranges, sized to fill whole
+// waves of the persistent grid.
 void gemm_ar_acc(const SliceStack& A, const SliceStack& B, double* C, long ldc, bool symmetric, cudaStream_t st)
 {
     if (A.Kp != B.Kp || A.ns != B.ns) throw std::runtime_error("i8gemm_ar_acc: operand stacks disagree");
-    if (A.ns * AR_BN > 512) throw std::runtime_error("i8gemm_ar_acc: too many slices for TMEM");
-    static bool configured = false;
-    static int nsm = 148;
-    if (!configured) {
-        CK(cudaFuncSetAttribute(i8gemm_ar_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AR_SMEM_MAX));
-        int dev = 0;
-        CK(cudaGetDevice(&dev));
-        CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-        configured = true;
-    }
-    int nsa = AR_MAXA;
-    while (nsa > 2 && ar_smem_bytes(nsa, A.ns) > AR_SMEM_MAX) nsa--;
+    if (A.ns < 1 || A.ns > MAXS) throw std::runtime_error("i8gemm_ar_acc: slice count out of range");
+    const int nsm = sm_count();
     CUtensorMap ta, tb;
     make_tmap(&ta, A.q, (uint64_t)A.ns * A.Rp, A.Kp, BM);
-    make_tmap(&tb, B.q, (uint64_t)B.ns * B.Rp, B.Kp, AR_BN);
+    make_tmap(&tb, B.q, (uint64_t)B.ns * B.Rp, B.Kp, BN);
     GemmParams P{};
     P.M = A.R; P.N = B.R; P.Kp = A.Kp; P.Mp = A.Rp; P.Np = B.Rp; P.ns = A.ns; P.symmetric = symmetric ? 1 : 0;
-    P.Ea = A.E; P.Eb = B.E; P.C = C; P.ldc = ldc; P.inner = 0; P.a_row0 = 0; P.ksplit = 1; P.dbg = nullptr;
-    P.stack = 1; P.nsa = nsa; P.accumulate = 1;
-    const int ntm = (A.R + BM - 1) / BM, ntn = (B.R + AR_BN - 1) / AR_BN;
+    P.Ea = A.E; P.Eb = B.E; P.C = C; P.ldc = ldc; P.inner = 0; P.a_row0 = 0; P.accumulate = 1;
+    const int ntm = (A.R + BM - 1) / BM, ntn = (B.R + BN - 1) / BN;
     int tiles = 0;
-    for (int mt = 0; mt < ntm; mt++) tiles += symmetric ? std::max(0, ntn - (BM / AR_BN) * mt) : ntn;
-    if (symmetric && ntn < (BM / AR_BN) * (ntm - 1) + 1) throw std::runtime_error("i8gemm_ar_acc: symmetric product needs a square output");
+    for (int mt = 0; mt < ntm; mt++) tiles += symmetric ? std::max(0, ntn - (BM / BN) * mt) : ntn;
+    if (symmetric && ntn < (BM / BN) * (ntm - 1) + 1) throw std::runtime_error("i8gemm_ar_acc: symmetric product needs a square output");
     const int nkb = A.Kp / BK;
     // K ranges: >= 8 K blocks each; among those the count that wastes the least of the last wave of the persistent grid
     int best = 1; double best_eff = -1.0;
@@ -263,56 +252,19 @@ void gemm_ar_acc(const SliceStack& A, const SliceStack& B, double* C, long ldc, 
         if (eff > best_eff + 1e-9) { best_eff = eff; best = kse; }
         if (items > 12L * nsm) break;
     }
-    static const int ks_env = getenv("B200JK_G2_KS") ? atoi(getenv("B200JK_G2_KS")) : 0;   // tuning experiment: force the K-range count
-    if (ks_env > 0) best = std::min(ks_env, std::max(1, nkb));
-    P.ar_kb_per = (nkb + best - 1) / best;
-    P.ar_ksplit = (nkb + P.ar_kb_per - 1) / P.ar_kb_per;
-    P.ar_ntiles = tiles;
-    const long items = (long)tiles * P.ar_ksplit;
-    dim3 grid((unsigned)std::min<long>(items, nsm));
-    i8gemm_ar_kernel<<<grid, NTHREADS, ar_smem_bytes(nsa, A.ns), st>>>(ta, tb, P);
-    CK(cudaGetLastError());
-}
-
-void gemm(const SliceStack& A, const SliceStack& B, double* C, long ldc, int inner, bool symmetric, cudaStream_t st, long long* dbg)
-{
-    if (A.Kp != B.Kp || A.ns != B.ns) throw std::runtime_error("i8gemm: operand stacks disagree");
-    static bool configured = false;
-    if (!configured) {
-        CK(cudaFuncSetAttribute(i8gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-        configured = true;
-    }
-    CUtensorMap ta, tb;
-    make_tmap(&ta, A.q, (uint64_t)A.ns * A.Rp, A.Kp, BM);
-    make_tmap(&tb, B.q, (uint64_t)B.ns * B.Rp, B.Kp, BN);
-    GemmParams P{};
-    P.M = A.R; P.N = B.R; P.Kp = A.Kp; P.Mp = A.Rp; P.Np = B.Rp; P.ns = A.ns; P.symmetric = symmetric ? 1 : 0;
-    P.Ea = A.E; P.Eb = B.E; P.C = C; P.ldc = ldc; P.inner = inner; P.dbg = dbg; P.a_row0 = 0;
-    const int mtiles = (A.R + BM - 1) / BM, ntiles = (B.R + BN - 1) / BN;
-    int tiles = 0;
-    for (int mt = 0; mt < mtiles; mt++)
-        for (int nt = 0; nt < ntiles; nt++)
-            if (!(symmetric && (nt + 1) * BN <= mt * BM)) tiles++;
-    int nkb = A.Kp / BK;
-    // split K so that the CTAs fill one (or two) waves of 148 SMs as exactly as possible, >= 8 K blocks each
-    int ksplit = 1, best_waste = 1 << 30;
-    for (int ks = 1; ks <= 64 && ks * 8 <= std::max(nkb, 8); ks++) {
-        int ctas = tiles * ks, waves = (ctas + 147) / 148;
-        if (waves > 2) break;
-        int waste = (waves * 148 - ctas) * 1000 / (waves * 148);
-        if (waste < best_waste || (waste == best_waste && ks > ksplit)) { best_waste = waste; ksplit = ks; }
-    }
-    P.ksplit = ksplit;
-    dim3 grid((B.R + BN - 1) / BN, (A.R + BM - 1) / BM, ksplit);
-    i8gemm_kernel<<<grid, NTHREADS, SMEM_BYTES, st>>>(ta, tb, P);
-    CK(cudaGetLastError());
+    P.kb_per = (nkb + best - 1) / best;
+    P.ksplit = (nkb + P.kb_per - 1) / P.kb_per;
+    P.ntiles = tiles;
+    const long items = (long)tiles * P.ksplit;
+    launch((unsigned)std::min<long>(items, nsm), ta, tb, P, st);
 }
 
 }  // namespace i8g
 }  // namespace b200jk
 #endif
 
-// C = A B^T through the tcgen05 int8-slice path; A [M,K], B [N,K], C [M,N] host fp64 (self-test / tests).
+// C = A B^T through the int8-slice tensor-core path; A [M,K], B [N,K], C [M,N] host fp64 (self-test / tests).
+// symmetric: only the upper triangle of C (M == N) is computed, the rest stays zero.
 extern "C" int b200jk_i8gemm_test(b200jk_handle h, int M, int N, int K, const double* A, const double* B, double* C, int ns,
                                   int symmetric)
 {
@@ -333,20 +285,10 @@ extern "C" int b200jk_i8gemm_test(b200jk_handle h, int M, int N, int K, const do
         split_rows(SA, dA, K, M, K, ns, st);
         split_rows(SB, dB, K, N, K, ns, st);
         CK(cudaEventRecord(h->ev0, st));
-        long long* ddbg = (long long*)dev_alloc(64 * 8);
-        dev_zero(ddbg, 64 * 8, st);
-        gemm(SA, SB, dC, N, 0, symmetric != 0, st, ddbg);
+        gemm_ar_acc(SA, SB, dC, N, symmetric != 0, st);
         CK(cudaEventRecord(h->ev1, st));
         d2h(C, dC, (size_t)M * N * 8, st);
-        long long hd[64];
-        d2h(hd, ddbg, 64 * 8, st);
         CK(cudaStreamSynchronize(st));
-        if (getenv("B200JK_I8_DEBUG")) {
-            fprintf(stderr, "i8gemm cycles (CTA 0,0) rel. to start:");
-            for (int i = 8; i < 8 + 4 * ns; i++) fprintf(stderr, "%s%lld", (i % 4 == 0) ? " | " : " ", hd[i] ? hd[i] - hd[0] : -1);
-            fprintf(stderr, "\n");
-        }
-        dev_free(ddbg);
         float ms = 0;
         CK(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
         h->stats.ms_kernels = ms;
@@ -356,7 +298,7 @@ extern "C" int b200jk_i8gemm_test(b200jk_handle h, int M, int N, int K, const do
     return 0;
 #else
     (void)M; (void)N; (void)K; (void)A; (void)B; (void)C; (void)ns; (void)symmetric;
-    set_err(h, "tcgen05 path is not emulated on the CPU");
+    set_err(h, "the tensor-core GEMM is not emulated on the CPU");
     return 3;
 #endif
 }

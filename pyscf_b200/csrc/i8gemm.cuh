@@ -1,16 +1,16 @@
-// i8gemm.cuh — FP64-accurate GEMM on the 5th-generation tensor cores (tcgen05, kind::i8) by error-free
-// slicing (Ozaki scheme): the DF-K contractions of pyscf/df/df_jk.py:373-380 (AO2MOnr_e2_drv's dsymm and
-// lib.dot/NPdgemm) executed as exact int8 x int8 -> int32 slice products.
+// i8gemm.cuh — FP64-accurate GEMM on the Hopper tensor cores (wgmma, s8 x s8 -> s32) by error-free slicing (Ozaki
+// scheme): the DF-K contractions of pyscf/df/df_jk.py:373-380 (AO2MOnr_e2_drv's dsymm and lib.dot/NPdgemm) executed as exact
+// int8 x int8 -> int32 slice products.
 //
 //   C[m,n] (+)= sum_k A[m,k] B[n,k]            A: [M,K], B: [N,K] fp64, both K-major (row-major, K contiguous)
 //
-// 1. split_rows_kernel: every row is scaled by 2^-E (E = ceil(log2 max|row|)) and cut into NS signed 7-bit slices
+// 1. the slicing kernels below scale every row by 2^-E (E = ceil(log2 max|row|)) and cut it into NS signed 7-bit slices
 //        a = 2^E ( q0 2^-6 + q1 2^-13 + ... + q_{NS-1} 2^-(6+7(NS-1)) ) + tail,  |q| <= 64.
-// 2. i8gemm_kernel: for every slice-pair group g = k+l (same power of two) the products A_k B_l^T are
-//    accumulated EXACTLY in a TMEM int32 accumulator by tcgen05.mma.kind::i8 (operands TMA-loaded into
-//    128B-swizzled shared memory through a 4-stage mbarrier ring); the epilogue warps read the accumulator
-//    back with tcgen05.ld, convert to fp64, apply 2^(Ea[m]+Eb[n]-12-7g) and add into C.  Two TMEM
-//    accumulators (2 x 256 columns) let the epilogue of group g overlap the MMAs of group g+1.
+// 2. i8gemm_kernel: for every slice-pair group g = k+l (same power of two) the products A_k B_l^T are accumulated EXACTLY
+//    in int32 registers by wgmma.mma_async (operands TMA-loaded into 128B-swizzled shared memory through mbarrier rings);
+//    all groups of a tile stay resident, each A_k tile is multiplied once with its stacked B slices.  The groups are then
+//    converted to fp64, weighted by 2^(-12-7g) and summed, smallest weight first; the epilogue applies the row / column
+//    exponents 2^(Ea[m]+Eb[n]) once per output element.
 // Only pairs with k+l < NS are formed (the rest is below the slice truncation): NS(NS+1)/2 slice GEMMs.
 #pragma once
 #include <cuda.h>
@@ -20,36 +20,34 @@
 namespace b200jk {
 namespace i8g {
 
-constexpr int BM = 128;        // UMMA M (cta_group::1)
-constexpr int BN = 256;        // UMMA N
+constexpr int BM = 128;        // rows of an output tile: two consumer warpgroups of 64 rows (wgmma M = 64)
+constexpr int BN = 32;         // columns of an output tile = rows of one B slice tile
 constexpr int BK = 128;        // bytes (= int8 elements) of K per pipeline stage: one 128B swizzle row
-constexpr int UK = 32;         // K per tcgen05.mma.kind::i8
-constexpr int NSTAGE = 4;
+constexpr int UK = 32;         // K per wgmma (s8)
 constexpr int MAXS = 8;        // max slices
+constexpr int NSA = 8;         // depth of the A ring (one A_k slice tile per stage)
+constexpr int NSB = 2;         // depth of the B ring (all ns slices of one K block per stage)
 constexpr int A_STAGE_BYTES = BM * BK;
-constexpr int B_STAGE_BYTES = BN * BK;
-constexpr int EPI_STAGE_INTS = 32 * 33;   // per epilogue warp: 32x32 int32 transpose buffer, padded
-constexpr int SMEM_BYTES = NSTAGE * (A_STAGE_BYTES + B_STAGE_BYTES) + 4 * EPI_STAGE_INTS * 4 + 1024 /*align*/ + 256 /*barriers*/;
-constexpr int NTHREADS = 192;  // warp0 TMA, warp1 MMA + TMEM alloc, warps 2..5 epilogue
+constexpr int B_SLICE_BYTES = BN * BK;
+constexpr int BAR_BYTES = 256;
+__host__ __device__ constexpr int smem_bytes(int ns) { return NSA * A_STAGE_BYTES + NSB * ns * B_SLICE_BYTES + BAR_BYTES + 1024 /*align*/; }
+constexpr int NTHREADS = 384;  // warpgroup 0: TMA producer (one thread), warpgroups 1, 2: wgmma + epilogue (64 rows each)
+constexpr int NCONSUMER_WARPS = 8;
 
 struct GemmParams {
     int M, N, Kp;          // Kp: padded K (multiple of BK)
     int Mp, Np;            // padded rows of the slice stacks (multiples of BM / BN)
     int ns;                // slices
-    int symmetric;         // 1: B == A, only tiles with n-tile >= m-tile*(BM/BN...) are computed (upper part)
+    int symmetric;         // 1: only tiles touching the upper triangle are computed, only elements n >= m are written
     const int* Ea; const int* Eb;   // per-row exponents
     double* C; long ldc;   // fp64 output, row-major [M, ldc]
     // optional transposed-scatter epilogue (stage 1 of DF-K): C element (m, n) is stored at
     //   C[(m % inner) * ldc + (m / inner) * N + n]   when inner > 0
     int inner;
     int a_row0;            // first row of the A stack used by this GEMM (row blocks of a persistent stack)
-    int ksplit;            // K blocks are divided among gridDim.z CTAs (fp64 reductions make this safe)
-    long long* dbg;        // optional cycle stamps of CTA (0,0) (tests/tuning)
-    int stack;             // i8gemm_ar_kernel: multiply A_k with up to 4 stacked B slices per MMA (N = 256)
-    int nsa;               // i8gemm_ar_kernel: depth of the A ring (host: as many 16 KB stages as fit in 227 KB)
-    // i8gemm_ar_kernel as stage 2 of DF-K (K += Y Y^T / Y G^T): work item = (tile, K range); ar_ksplit K ranges per tile,
-    // results meet in fp64 reductions (accumulate), only tiles touching the upper triangle when symmetric
-    int ar_ksplit, ar_kb_per, ar_ntiles, accumulate;
+    // work item = (tile, K range); ksplit K ranges of kb_per K blocks per tile, ntiles tiles.  Partial results of the K ranges
+    // meet in fp64 reductions (accumulate)
+    int ksplit, kb_per, ntiles, accumulate;
     // stage 1: optional per-output-row maxima (bit pattern of max |C| per row m % inner, 64-bit atomicMax), so that the slicing
     // of Y needs no row-maximum pass of its own
     unsigned long long* rowmax;
@@ -91,7 +89,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity)
 }
 __device__ __forceinline__ double pow2i(int e) { return __longlong_as_double((long long)(e + 1023) << 52); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int c0, int c1)
 {
@@ -104,63 +101,64 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tmap)
     asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t ncols)
-{
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t ncols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem]^T, int8 x int8 -> int32
-__device__ __forceinline__ void mma_i8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate)
+// d[64 x N] += A[64 x 32] * B[N x 32]^T, s8 x s8 -> s32, both operands K-major in shared memory.
+// Fragment of thread t of the warpgroup: d[4j + 2i + c] = D[16 (t/32) + (t%32)/4 + 8i][8j + 2(t%4) + c], j < N/8.
+template <int N>
+__device__ __forceinline__ void wgmma_s8(int32_t* d, uint64_t desc_a, uint64_t desc_b);
+template <> __device__ __forceinline__ void wgmma_s8<32>(int32_t* d, uint64_t desc_a, uint64_t desc_b)
 {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\twgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+                 : "l"(desc_a), "l"(desc_b), "r"(1));
 }
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void mma_commit(uint64_t* bar)
+template <> __device__ __forceinline__ void wgmma_s8<64>(int32_t* d, uint64_t desc_a, uint64_t desc_b)
 {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\twgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n\t}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+                 : "l"(desc_a), "l"(desc_b), "r"(1));
 }
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32])
+template <> __device__ __forceinline__ void wgmma_s8<96>(int32_t* d, uint64_t desc_a, uint64_t desc_b)
 {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\twgmma.mma_async.sync.aligned.m64n96k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p;\n\t}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47])
+                 : "l"(desc_a), "l"(desc_b), "r"(1));
+}
+template <> __device__ __forceinline__ void wgmma_s8<128>(int32_t* d, uint64_t desc_a, uint64_t desc_b)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\twgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n\t}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+                 : "l"(desc_a), "l"(desc_b), "r"(1));
+}
+template <> __device__ __forceinline__ void wgmma_s8<160>(int32_t* d, uint64_t desc_a, uint64_t desc_b)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %82, 0;\n\twgmma.mma_async.sync.aligned.m64n160k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, %80, %81, p;\n\t}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]), "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]), "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79])
+                 : "l"(desc_a), "l"(desc_b), "r"(1));
+}
+template <> __device__ __forceinline__ void wgmma_s8<192>(int32_t* d, uint64_t desc_a, uint64_t desc_b)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\twgmma.mma_async.sync.aligned.m64n192k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, %96, %97, p;\n\t}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]), "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]), "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]), "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]), "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95])
+                 : "l"(desc_a), "l"(desc_b), "r"(1));
+}
+template <> __device__ __forceinline__ void wgmma_s8<224>(int32_t* d, uint64_t desc_a, uint64_t desc_b)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %114, 0;\n\twgmma.mma_async.sync.aligned.m64n224k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111}, %112, %113, p;\n\t}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]), "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]), "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]), "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]), "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]), "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]), "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111])
+                 : "l"(desc_a), "l"(desc_b), "r"(1));
+}
+template <> __device__ __forceinline__ void wgmma_s8<256>(int32_t* d, uint64_t desc_a, uint64_t desc_b)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\twgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p;\n\t}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]), "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]), "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]), "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]), "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]), "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]), "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]), "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]), "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
+                 : "l"(desc_a), "l"(desc_b), "r"(1));
 }
 
-// the same load without the wait: several loads in flight, then one tmem_ld_wait()
-__device__ __forceinline__ void tmem_ld_32x32b_x32_nowait(uint32_t taddr, uint32_t (&r)[32])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 // exact int32 -> fp64 on the FP64 add pipe (one LOP + one DADD instead of a conversion instruction):
 // the double with high word 0x43300000 and low word (x ^ 2^31) is 2^52 + 2^31 + x
 __device__ __forceinline__ double i2d_exact(uint32_t x)
@@ -168,449 +166,236 @@ __device__ __forceinline__ double i2d_exact(uint32_t x)
     return __hiloint2double(0x43300000, (int)(x ^ 0x80000000u)) - 4503601774854144.0;
 }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp SmemDescriptor):
-// start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48) | layout SWIZZLE_128B=2 [61,64)
+// K-major, 128B-swizzled shared-memory matrix descriptor of wgmma:
+// start>>4 [0,14) | LBO>>4 [16,30) (unused for swizzled K-major, canonical 1) | SBO>>4 [32,46): 8 rows x 128 B between
+// row groups | layout type [62,64): 1 = SWIZZLE_128B.  The tile base is 1024-byte aligned; the K offset inside the swizzle
+// row is added to the start address.
 __device__ __forceinline__ uint64_t make_desc_k_sw128(uint32_t smem_addr)
 {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;                 // leading byte offset (unused for swizzled K-major), canonical value 1
-    d |= (uint64_t)(1024 >> 4) << 32;       // stride byte offset: 8 rows x 128 B between row groups
-    d |= (uint64_t)1 << 46;                 // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                 // SWIZZLE_128B
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// instruction descriptor for kind::i8: c=S32, a=b=INT8, both K-major, N>>3 at [17,23), M>>4 at [24,29)
-__host__ __device__ constexpr uint32_t make_idesc_i8(int m, int n)
+
+// work item -> (m tile, n tile, K-block range).  Items are numbered K range slowest, tile fastest (CTAs running side by side
+// share the A tile of their m tile in L2); symmetric: only the tiles with (nt + 1) * BN > mt * BM, i.e. nt >= 2 mt.
+__device__ __forceinline__ void decode_item(const GemmParams& P, int item, int ntn, int nkb, int& mt, int& nt, int& kb0, int& kb1)
 {
-    return (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+    const int ks = item / P.ntiles;
+    int tile = item - ks * P.ntiles;
+    if (P.symmetric) {
+        mt = 0;
+        for (;;) {
+            const int cnt = ntn - (BM / BN) * mt;
+            if (tile < cnt) break;
+            tile -= cnt; mt++;
+        }
+        nt = (BM / BN) * mt + tile;
+    } else {
+        mt = tile / ntn; nt = tile - mt * ntn;
+    }
+    kb0 = ks * P.kb_per;
+    kb1 = (kb0 + P.kb_per < nkb) ? kb0 + P.kb_per : nkb;
 }
 
 // ---------------------------------------------------------------------------------------------- GEMM kernel
+// One K block of a consumer warpgroup, A slices k = K .. NS-1 (compile-time k and l: straight-line code).  A_k (64 rows of this
+// warpgroup) times each B slice l = 0 .. NS-1-k: one m64n32k32 wgmma per pair and 32 bytes of K into the accumulator of group
+// k + l (acc[16 (k + l)] .. +15).  Every wgmma has the same shape and writes one whole, disjoint 16-register block, so ptxas
+// keeps them in flight (mixed shapes over overlapping sub-ranges of acc serialise the wgmma pipeline).  The A stage of slice
+// k-1 is handed back as soon as the products of slice k are issued behind it.
+template <int NS, int K>
+struct SliceMMA {
+    static __device__ __forceinline__ void run(int32_t* acc, uint8_t* sA, uint64_t* afull, uint64_t* aempty, uint32_t b0, int h,
+                                               int lane, int& sa, uint32_t& pa, int prev)
+    {
+        mbar_wait(&afull[sa], pa);
+        const uint32_t a0 = smem_u32(sA + sa * A_STAGE_BYTES + h * (BM / 2) * BK);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < BK / UK; kk++)
+#pragma unroll
+            for (int l = 0; l < NS - K; l++)
+                wgmma_s8<BN>(acc + (BN / 2) * (K + l), make_desc_k_sw128(a0 + kk * UK), make_desc_k_sw128(b0 + l * B_SLICE_BYTES + kk * UK));
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (K > 0 && lane == 0) mbar_arrive(&aempty[prev]);
+        const int cur = sa;
+        if (++sa == NSA) { sa = 0; pa ^= 1; }
+        SliceMMA<NS, K + 1>::run(acc, sA, afull, aempty, b0, h, lane, sa, pa, cur);
+    }
+};
+template <int NS>
+struct SliceMMA<NS, NS> {
+    static __device__ __forceinline__ void run(int32_t*, uint8_t*, uint64_t*, uint64_t* aempty, uint32_t, int, int lane, int&,
+                                               uint32_t&, int prev)
+    {
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&aempty[prev]);
+    }
+};
+
 // tmapA / tmapB: 2-D uint8 tensors [ns*Mp (resp. ns*Np) rows][Kp bytes], box {BK, BM} / {BK, BN}, SWIZZLE_128B.
+// Persistent: CTA b takes the work items b, b + gridDim.x, ...  Per K block of an item the producer loads the NS slices of the
+// B tile once (back to back: rows l*BN of the stage form one K-major operand of NS*BN rows) and the NS slice tiles A_k one after
+// the other; all NS(NS+1)/2 slice products of the K block are formed from these loads (A-stationary: no operand is re-read).
+// The epilogue is one of
+//   yq:         the int8 slices of Y are cut from the fp64 tile (stage 1 of DF-K, Y never exists in fp64),
+//   accumulate: fp64 reductions into C (stage 2 of DF-K, K ranges of one tile meet there),
+//   otherwise:  plain stores into C (+ row maxima).
+template <int NS>
 __global__ void __launch_bounds__(NTHREADS, 1)
 i8gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB, const GemmParams P)
 {
     extern __shared__ uint8_t smem_raw[];
-    // 1024-byte alignment for SWIZZLE_128B
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // 1024-byte aligned, still known to be shared memory
+    constexpr int B_STAGE_BYTES = NS * B_SLICE_BYTES;
     uint8_t* sA = smem;
-    uint8_t* sB = smem + NSTAGE * A_STAGE_BYTES;
-    uint64_t* bars = (uint64_t*)(smem + NSTAGE * (A_STAGE_BYTES + B_STAGE_BYTES));
-    uint64_t* full = bars;                 // [NSTAGE]
-    uint64_t* empty = bars + NSTAGE;       // [NSTAGE]
-    uint64_t* tfull = bars + 2 * NSTAGE;   // [2]
-    uint64_t* tempty = bars + 2 * NSTAGE + 2;  // [2]
-    uint32_t* tmem_slot = (uint32_t*)(bars + 2 * NSTAGE + 4);
-    int* epi_stage = (int*)(smem + NSTAGE * (A_STAGE_BYTES + B_STAGE_BYTES) + 256);
+    uint8_t* sB = smem + NSA * A_STAGE_BYTES;
+    uint64_t* afull = (uint64_t*)(sB + NSB * B_STAGE_BYTES);   // [NSA] operands landed (TMA -> wgmma)
+    uint64_t* aempty = afull + NSA;                              // [NSA] stage consumed (wgmma -> TMA), one arrival per consumer warp
+    uint64_t* bfull = aempty + NSA;                              // [NSB]
+    uint64_t* bempty = bfull + NSB;                              // [NSB]
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int mt = blockIdx.y, nt = blockIdx.x;
-    if (P.symmetric && (nt + 1) * BN <= mt * BM) return;   // tile entirely below the diagonal
-    const int nkb_all = P.Kp / BK;
-    const int kb_per = (nkb_all + P.ksplit - 1) / P.ksplit;
-    const int kb0 = blockIdx.z * kb_per;
-    const int kb1 = (kb0 + kb_per < nkb_all) ? kb0 + kb_per : nkb_all;
-    const int nkb = kb1 - kb0;
-    if (nkb <= 0) return;
-    const int ns = P.ns;
-
-    if (warp == 0 && lane == 0) {
-        prefetch_tmap(&tmapA);
-        prefetch_tmap(&tmapB);
-        for (int i = 0; i < NSTAGE; i++) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        for (int i = 0; i < 2; i++) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 4); }
-        fence_barrier_init();
-    }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const bool dbg_on = P.dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
-    if (dbg_on && threadIdx.x == 0) P.dbg[0] = clock64();
-
-    if (warp == 0) {
-        // ===== TMA producer =====
-        if (lane == 0) {
-            int stage = 0; uint32_t phase = 0;
-            for (int g = ns - 1; g >= 0; g--)
-                for (int k = 0; k <= g; k++) {
-                    const int l = g - k;
-                    for (int kb = 0; kb < nkb; kb++) {
-                        mbar_wait(&empty[stage], phase ^ 1);
-                        mbar_expect_tx(&full[stage], A_STAGE_BYTES + B_STAGE_BYTES);
-                        tma_load_2d(sA + stage * A_STAGE_BYTES, &tmapA, &full[stage], (kb0 + kb) * BK, k * P.Mp + P.a_row0 + mt * BM);
-                        tma_load_2d(sB + stage * B_STAGE_BYTES, &tmapB, &full[stage], (kb0 + kb) * BK, l * P.Np + nt * BN);
-                        if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-                    }
-                }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer (one elected thread) =====
-        if (lane == 0) {
-            constexpr uint32_t idesc = make_idesc_i8(BM, BN);
-            int stage = 0; uint32_t phase = 0;
-            int it = 0;
-            for (int g = ns - 1; g >= 0; g--, it++) {
-                const int buf = it & 1;
-                const uint32_t tphase = (it >> 1) & 1;
-                mbar_wait(&tempty[buf], tphase ^ 1);          // epilogue has drained this accumulator
-                if (dbg_on) P.dbg[8 + 4 * it] = clock64();
-                tc_fence_after();
-                const uint32_t tacc = tmem_base + buf * BN;
-                uint32_t acc = 0;
-                for (int k = 0; k <= g; k++)
-                    for (int kb = 0; kb < nkb; kb++) {
-                        mbar_wait(&full[stage], phase);
-                        tc_fence_after();
-                        const uint32_t a0 = smem_u32(sA + stage * A_STAGE_BYTES), b0 = smem_u32(sB + stage * B_STAGE_BYTES);
-#pragma unroll
-                        for (int kk = 0; kk < BK / UK; kk++) {
-                            mma_i8(tacc, make_desc_k_sw128(a0 + kk * UK), make_desc_k_sw128(b0 + kk * UK), idesc, acc);
-                            acc = 1;
-                        }
-                        mma_commit(&empty[stage]);            // frees the smem stage when these MMAs retire
-                        if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-                    }
-                mma_commit(&tfull[buf]);                      // accumulator of group g complete
-                if (dbg_on) P.dbg[9 + 4 * it] = clock64();
-            }
-        }
-    } else {
-        // ===== epilogue warps: TMEM -> registers -> smem transpose -> coalesced fp64 read-modify-write of C =====
-        const int q = warp & 3;                  // TMEM lane quarter this warp may access
-        int* stg = epi_stage + q * EPI_STAGE_INTS;
-        const int mrow0 = mt * BM + q * 32;      // first row of this warp's 32-row band
-        int it = 0;
-        for (int g = ns - 1; g >= 0; g--, it++) {
-            const int buf = it & 1;
-            const uint32_t tphase = (it >> 1) & 1;
-            mbar_wait(&tfull[buf], tphase);
-            tc_fence_after();
-            if (dbg_on && q == 0 && lane == 0) P.dbg[10 + 4 * it] = clock64();
-            const int eg = -12 - 7 * g;
-#pragma unroll 1
-            for (int c0 = 0; c0 < BN; c0 += 32) {
-                uint32_t r[32];
-                tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + buf * BN + c0, r);
-                const int n = nt * BN + c0 + lane;       // this lane's column after the transpose
-                if (nt * BN + c0 >= P.N) continue;
-#pragma unroll
-                for (int j = 0; j < 32; j++) stg[lane * 33 + j] = (int)r[j];
-                __syncwarp();
-                const bool ncol_ok = n < P.N;
-                const int ebn = ncol_ok ? __ldg(P.Eb + n) : 0;
-#pragma unroll 4
-                for (int rr = 0; rr < 32; rr++) {
-                    const int m = mrow0 + rr;
-                    if (m >= P.M) break;
-                    if (ncol_ok && (!P.symmetric || n >= m)) {
-                        // __ldg: a plain load could not be hoisted above the preceding reduction (possible alias) and the
-                        // 32 rows would serialise on the load latency
-                        const double v = (double)stg[rr * 33 + lane] * pow2i(__ldg(P.Ea + P.a_row0 + m) + ebn + eg);
-                        double* dst;
-                        if (P.inner > 0) dst = P.C + (long)(m % P.inner) * P.ldc + (long)(m / P.inner) * P.N + n;
-                        else dst = P.C + (long)m * P.ldc + n;
-                        atomicAdd(dst, v);   // RED.ADD.F64: no read latency, safe under split-K
-                    }
-                }
-                __syncwarp();
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (dbg_on && q == 0 && lane == 0) P.dbg[11 + 4 * it] = clock64();
-            if (lane == 0) mbar_arrive(&tempty[buf]);
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 512);
-}
-
-// ---------------------------------------------------------------------------------------------- GEMM kernel, "all groups resident"
-// Variant for a SHORT contraction (K = nao) and a narrow N (stage 1 of DF-K: N = nocc): tile 128 x 64 with ALL slice-pair
-// groups resident in TMEM (group g at columns g*64, ns*64 <= 512).  The A_k tile is loaded ONCE per (K block, k) and
-// reused for every B_l (A-stationary: no operand re-reads), and there is ONE epilogue per tile that combines the groups in
-// fp64 registers and stores each output once (no read-modify-write, no zero fill).
-// Persistent: one CTA per SM walks over the tiles (N tile fastest, so the CTAs that share an A tile run side by side
-// and meet in L2).  The TMA producer keeps prefetching the next tile's operands while the epilogue drains TMEM; the
-// accumulators are handed back to the MMA warp as soon as the last tcgen05.ld has landed, before the stores.
-constexpr int AR_BN = 64;
-constexpr int AR_NSB = 2;                        // B ring: ALL slices of a K block per stage
-constexpr int AR_MAXA = 8;                       // A ring: one slice tile per stage, depth chosen by the host (P.nsa)
-constexpr int AR_A_BYTES = BM * BK, AR_B1_BYTES = AR_BN * BK;
-constexpr int AR_BAR_BYTES = 512, AR_EPI_BYTES = 0;   // the epilogue needs no staging: every lane stores its own row
-constexpr int AR_SMEM_MAX = 232448;              // 227 KB opt-in limit per CTA
-__host__ __device__ constexpr int ar_smem_bytes(int nsa, int ns) { return nsa * AR_A_BYTES + AR_NSB * ns * AR_B1_BYTES + AR_BAR_BYTES + AR_EPI_BYTES + 1024; }
-
-// work item -> (m tile, n tile, K-block range).  Items are numbered K range slowest, tile fastest (CTAs running side by side
-// share the A tile of their m tile in L2); symmetric: only the tiles with (nt + 1) * AR_BN > mt * BM, i.e. nt >= 2 mt.
-__device__ __forceinline__ void ar_decode_item(const GemmParams& P, int item, int ntn, int nkb, int& mt, int& nt, int& kb0, int& kb1)
-{
-    const int ks = item / P.ar_ntiles;
-    int tile = item - ks * P.ar_ntiles;
-    if (P.symmetric) {
-        mt = 0;
-        for (;;) {
-            const int cnt = ntn - (BM / AR_BN) * mt;
-            if (tile < cnt) break;
-            tile -= cnt; mt++;
-        }
-        nt = (BM / AR_BN) * mt + tile;
-    } else {
-        mt = tile / ntn; nt = tile - mt * ntn;
-    }
-    kb0 = ks * P.ar_kb_per;
-    kb1 = (kb0 + P.ar_kb_per < nkb) ? kb0 + P.ar_kb_per : nkb;
-}
-
-__global__ void __launch_bounds__(NTHREADS, 1)
-i8gemm_ar_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB, const GemmParams P)
-{
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // 1024-byte aligned, still known to be shared memory
-    const int ns = P.ns, nsa = P.nsa;
-    const int bstage = ns * AR_B1_BYTES;
-    uint8_t* sA = smem;
-    uint8_t* sB = smem + nsa * AR_A_BYTES;
-    uint64_t* bars = (uint64_t*)(sB + AR_NSB * bstage);
-    uint64_t* afull = bars;                      // [AR_MAXA]
-    uint64_t* aempty = afull + AR_MAXA;
-    uint64_t* bfull = aempty + AR_MAXA;          // [AR_NSB]
-    uint64_t* bempty = bfull + AR_NSB;
-    uint64_t* tfull = bempty + AR_NSB;           // [1] accumulators complete (MMA -> epilogue)
-    uint64_t* tempty = tfull + 1;                // [MAXS] accumulator of slice-pair group g drained (epilogue -> MMA), 4 arrivals each
-    uint32_t* tmem_slot = (uint32_t*)(tempty + MAXS);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
     const int nkb = P.Kp / BK;
-    const int ntn = (P.N + AR_BN - 1) / AR_BN, ntm = (P.M + BM - 1) / BM;
-    const int ntiles = P.ar_ntiles * P.ar_ksplit;     // work items
-    (void)ntm;
+    const int ntn = (P.N + BN - 1) / BN;
+    const int nitems = P.ntiles * P.ksplit;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         prefetch_tmap(&tmapA);
         prefetch_tmap(&tmapB);
-        for (int i = 0; i < nsa; i++) { mbar_init(&afull[i], 1); mbar_init(&aempty[i], 1); }
-        for (int i = 0; i < AR_NSB; i++) { mbar_init(&bfull[i], 1); mbar_init(&bempty[i], 1); }
-        mbar_init(tfull, 1);
-        for (int g = 0; g < MAXS; g++) mbar_init(&tempty[g], 4);
+        for (int i = 0; i < NSA; i++) { mbar_init(&afull[i], 1); mbar_init(&aempty[i], NCONSUMER_WARPS); }
+        for (int i = 0; i < NSB; i++) { mbar_init(&bfull[i], 1); mbar_init(&bempty[i], NCONSUMER_WARPS); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    // The A slices of a K block are taken in DESCENDING order k = ns-1 .. 0: slice k multiplies B slices 0 .. ns-1-k into the
-    // groups k .. ns-1, so group g is first touched by A_g, and the next tile's MMAs can start as soon as the epilogue has
-    // drained group ns-1 (it drains in the same order) instead of waiting for the whole accumulator.
-    if (warp == 0) {
-        if (lane == 0) {
+    if (wg == 0) {
+        // ===== TMA producer: hands its registers to the consumers (128 x 40 + 256 x 232 <= 64 K) =====
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+        if (threadIdx.x == 0) {
             int sa = 0, sb = 0; uint32_t pa = 0, pb = 0;
-            for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+            for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
                 int mt, nt, kb0, kb1;
-                ar_decode_item(P, tile, ntn, nkb, mt, nt, kb0, kb1);
+                decode_item(P, item, ntn, nkb, mt, nt, kb0, kb1);
                 for (int kb = kb0; kb < kb1; kb++) {
                     mbar_wait(&bempty[sb], pb ^ 1);
-                    mbar_expect_tx(&bfull[sb], ns * AR_B1_BYTES);
-                    for (int l = 0; l < ns; l++)
-                        tma_load_2d(sB + sb * bstage + l * AR_B1_BYTES, &tmapB, &bfull[sb], kb * BK, l * P.Np + nt * AR_BN);
-                    if (++sb == AR_NSB) { sb = 0; pb ^= 1; }
-                    for (int k = ns - 1; k >= 0; k--) {
+                    mbar_expect_tx(&bfull[sb], B_STAGE_BYTES);
+                    for (int l = 0; l < NS; l++)
+                        tma_load_2d(sB + sb * B_STAGE_BYTES + l * B_SLICE_BYTES, &tmapB, &bfull[sb], kb * BK, l * P.Np + nt * BN);
+                    if (++sb == NSB) { sb = 0; pb ^= 1; }
+                    for (int k = 0; k < NS; k++) {
                         mbar_wait(&aempty[sa], pa ^ 1);
-                        mbar_expect_tx(&afull[sa], AR_A_BYTES);
-                        tma_load_2d(sA + sa * AR_A_BYTES, &tmapA, &afull[sa], kb * BK, k * P.Mp + P.a_row0 + mt * BM);
-                        if (++sa == nsa) { sa = 0; pa ^= 1; }
+                        mbar_expect_tx(&afull[sa], A_STAGE_BYTES);
+                        tma_load_2d(sA + sa * A_STAGE_BYTES, &tmapA, &afull[sa], kb * BK, k * P.Mp + P.a_row0 + mt * BM);
+                        if (++sa == NSA) { sa = 0; pa ^= 1; }
                     }
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            int sa = 0, sb = 0; uint32_t pa = 0, pb = 0;
-            int it = 0;
-            for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, it++) {
-                if (P.dbg && blockIdx.x == 0 && it < 6) P.dbg[it * 8 + 0] = clock64();
-                int mt_, nt_, kb0, kb1;
-                ar_decode_item(P, tile, ntn, nkb, mt_, nt_, kb0, kb1);
-                for (int kb = kb0; kb < kb1; kb++) {
-                    mbar_wait(&bfull[sb], pb);
-                    tc_fence_after();
-                    const uint32_t bbase = smem_u32(sB + sb * bstage);
-                    for (int k = ns - 1; k >= 0; k--) {
-                        mbar_wait(&afull[sa], pa);
-                        if (kb == kb0) {
-                            mbar_wait(&tempty[k], (uint32_t)((it & 1) ^ 1));   // the epilogue has read group k of the previous tile
-                            if (k == ns - 1 && P.dbg && blockIdx.x == 0 && it < 6) P.dbg[it * 8 + 1] = clock64();
-                        }
-                        tc_fence_after();
-                        const uint32_t a0 = smem_u32(sA + sa * AR_A_BYTES);
-                        // The B slices l = 0..ns-1-k of this K block lie back to back in shared memory (64 rows x 128 B each),
-                        // i.e. they ARE one K-major tile of (ns-k)*64 rows, and their groups k+l are adjacent TMEM column
-                        // blocks: one MMA with N = 64*cnt multiplies A_k with cnt slices at once.  A 128-row MMA costs the
-                        // same ~128 cycles for any N <= 256, so stacking cuts the 28 slice-pair MMAs per K block to 10.
-                        // The first touch of group g is (kb = 0, k = g, l = 0) and has to overwrite: in the first K block that
-                        // pair gets an MMA of its own (N = 64), the stacked MMAs start at l = 1.
-                        const int lstep = P.stack ? 4 : 1;
-                        int l = 0;
-                        if (kb == kb0) {
-                            const uint32_t idesc_1 = make_idesc_i8(BM, AR_BN);
-                            const uint32_t tacc = tmem_base + k * AR_BN;
-                            uint32_t acc = 0;
+        return;
+    }
+
+    // ===== consumers: warpgroup h = wg - 1 owns rows 64 h .. 64 h + 63 of the tile; 16 NS accumulator registers per thread =====
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+    const int h = wg - 1;
+    const int t = threadIdx.x & 127;
+    const int rq = 16 * (t >> 5) + (lane >> 2);     // fragment rows rq, rq + 8 of this warpgroup's 64
+    const int cq = 2 * (lane & 3);                  // fragment columns 8j + cq, 8j + cq + 1
+    constexpr int NF = BN / 2;                      // accumulator registers per group
+    int sa = 0, sb = 0; uint32_t pa = 0, pb = 0;
+    for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
+        int mt, nt, kb0, kb1;
+        decode_item(P, item, ntn, nkb, mt, nt, kb0, kb1);
+        int32_t acc[NS * NF];
 #pragma unroll
-                            for (int kk = 0; kk < BK / UK; kk++) {
-                                mma_i8(tacc, make_desc_k_sw128(a0 + kk * UK), make_desc_k_sw128(bbase + kk * UK), idesc_1, acc);
-                                acc = 1;
-                            }
-                            l = 1;
-                        }
-                        for (; l < ns - k; l += lstep) {
-                            const int cnt = (ns - k - l < lstep) ? ns - k - l : lstep;
-                            const uint32_t idesc_n = make_idesc_i8(BM, cnt * AR_BN);
-                            const uint32_t b0 = bbase + l * AR_B1_BYTES;
-                            const uint32_t tacc = tmem_base + (k + l) * AR_BN;
-#pragma unroll
-                            for (int kk = 0; kk < BK / UK; kk++)
-                                mma_i8(tacc, make_desc_k_sw128(a0 + kk * UK), make_desc_k_sw128(b0 + kk * UK), idesc_n, 1u);
-                        }
-                        mma_commit(&aempty[sa]);
-                        if (++sa == nsa) { sa = 0; pa ^= 1; }
-                    }
-                    mma_commit(&bempty[sb]);
-                    if (++sb == AR_NSB) { sb = 0; pb ^= 1; }
-                }
-                mma_commit(tfull);
-                if (P.dbg && blockIdx.x == 0 && it < 6) P.dbg[it * 8 + 2] = clock64();   // all MMAs of the tile issued
-            }
+        for (int j = 0; j < NS * NF; j++) acc[j] = 0;
+        for (int kb = kb0; kb < kb1; kb++) {
+            mbar_wait(&bfull[sb], pb);
+            SliceMMA<NS, 0>::run(acc, sA, afull, aempty, smem_u32(sB + sb * B_STAGE_BYTES), h, lane, sa, pa, 0);
+            if (lane == 0) mbar_arrive(&bempty[sb]);
+            if (++sb == NSB) { sb = 0; pb ^= 1; }
         }
-    } else {
-        const int q = warp & 3;
-        int it = 0;
-        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, it++) {
-            int mt, nt, kb0_, kb1_;
-            ar_decode_item(P, tile, ntn, nkb, mt, nt, kb0_, kb1_);
-            const int mrow0 = mt * BM + q * 32;
-            // exponent and output offset of this warp's 32 rows, one row per lane, fetched once per tile (see i8gemm_kernel)
-            const int mlane = mrow0 + lane;
-            const int ea_lane = (mlane < P.M) ? __ldg(P.Ea + P.a_row0 + mlane) : 0;
-            const long off_lane = (P.inner > 0) ? (long)(mlane % P.inner) * P.ldc + (long)(mlane / P.inner) * P.N : (long)mlane * P.ldc;
-            const bool stamp = P.dbg && blockIdx.x == 0 && it < 6 && q == 0 && lane == 0;
-            if (stamp) P.dbg[it * 8 + 3] = clock64();
-            mbar_wait(tfull, (uint32_t)(it & 1));
-            tc_fence_after();
-            if (stamp) P.dbg[it * 8 + 4] = clock64();   // accumulators complete
-            // combine the groups in fp64, smallest weight first, row = this lane, all 64 columns; every group is handed back to
-            // the MMA warp as soon as its loads have landed
-            double accv[AR_BN];
+        double accv[NF];
 #pragma unroll
-            for (int j = 0; j < AR_BN; j++) accv[j] = 0.0;
-            const bool on0 = nt * AR_BN < P.N, on1 = nt * AR_BN + 32 < P.N;
-#pragma unroll 1
-            for (int g = ns - 1; g >= 0; g--) {
-                uint32_t r0[32], r1[32];
-                const uint32_t ta = tmem_base + ((uint32_t)(q * 32) << 16) + g * AR_BN;
-                if (on0) tmem_ld_32x32b_x32_nowait(ta, r0);
-                if (on1) tmem_ld_32x32b_x32_nowait(ta + 32, r1);
-                tmem_ld_wait();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tempty[g]);
-                const double w = pow2i(-12 - 7 * g);
-                if (on0) {
+        for (int j = 0; j < NF; j++) accv[j] = 0.0;
 #pragma unroll
-                    for (int j = 0; j < 32; j++) accv[j] += i2d_exact(r0[j]) * w;
-                }
-                if (on1) {
+        for (int g = NS - 1; g >= 0; g--) {
+            const double w = pow2i(-12 - 7 * g);
 #pragma unroll
-                    for (int j = 0; j < 32; j++) accv[32 + j] += i2d_exact(r1[j]) * w;
-                }
-            }
-            if (stamp) P.dbg[it * 8 + 5] = clock64();   // TMEM handed back
-            // lane = output row (the TMEM lane): its 64 columns are contiguous in C, so every lane streams its own 512 B;
-            // the partial sectors of neighbouring stores merge in L2.  No transpose, no shuffles; the column exponents come
-            // through the read-only path, so they are not ordered behind the stores of the previous row.
+            for (int j = 0; j < NF; j++) accv[j] += i2d_exact((uint32_t)acc[g * NF + j]) * w;
+        }
+
+        const int nb = nt * BN;
+#pragma unroll
+        for (int i = 0; i < 2; i++) {
+            const int m = mt * BM + h * (BM / 2) + rq + 8 * i;
+            if (m >= P.M) continue;
+            const int ea = __ldg(P.Ea + P.a_row0 + m);
             if (P.yq) {
                 // Y never exists in fp64: scale the row by its exponent bound and cut the balanced 7-bit digits here
                 // (round-to-nearest by the 1.5*2^52 trick: two adds per digit instead of a rounding and a conversion instruction)
-                if (mlane < P.M) {
-                    const int nb = nt * AR_BN;
-                    const int yrow = mlane % P.inner;
-                    const long ycol0 = (long)(mlane / P.inner) * P.y_ncolp + nb;
-                    const int esc = ea_lane + 6 - __ldg(P.Ey + yrow);
-                    int8_t* dst0 = P.yq + (long)yrow * P.y_Kp + ycol0;
-                    const long sstride = (long)P.y_Rp * P.y_Kp;
+                const int yrow = m % P.inner;
+                const long ycol0 = (long)(m / P.inner) * P.y_ncolp;
+                const int esc = ea + 6 - __ldg(P.Ey + yrow);
+                int8_t* dst0 = P.yq + (long)yrow * P.y_Kp + ycol0;
+                const long sstride = (long)P.y_Rp * P.y_Kp;
 #pragma unroll
-                    for (int j0 = 0; j0 < AR_BN; j0 += 16) {
-                        if (nb + j0 >= P.y_ncolp) break;
-                        double rr[16];
-#pragma unroll
-                        for (int j = 0; j < 16; j += 4) {
-                            const int4 eb = __ldg(reinterpret_cast<const int4*>(P.Eb + nb + j0 + j));
-                            rr[j] = accv[j0 + j] * pow2i(esc + eb.x); rr[j + 1] = accv[j0 + j + 1] * pow2i(esc + eb.y);
-                            rr[j + 2] = accv[j0 + j + 2] * pow2i(esc + eb.z); rr[j + 3] = accv[j0 + j + 3] * pow2i(esc + eb.w);
-                        }
-                        for (int s_ = 0; s_ < ns; s_++) {
-                            unsigned w[4];
-#pragma unroll
-                            for (int q4 = 0; q4 < 4; q4++) {
-                                unsigned pack = 0;
-#pragma unroll
-                                for (int j = 0; j < 4; j++) {
-                                    const double t_ = rr[4 * q4 + j] + 6755399441055744.0;
-                                    const double qv = t_ - 6755399441055744.0;
-                                    pack |= ((unsigned)__double2loint(t_) & 255u) << (8 * j);
-                                    rr[4 * q4 + j] = (rr[4 * q4 + j] - qv) * 128.0;
-                                }
-                                w[q4] = pack;
-                            }
-                            *reinterpret_cast<uint4*>(dst0 + s_ * sstride + j0) = make_uint4(w[0], w[1], w[2], w[3]);
-                        }
+                for (int j = 0; j < BN / 8; j++) {
+                    const int n = nb + 8 * j + cq;
+                    if (n >= P.y_ncolp) continue;    // y_ncolp is a multiple of 16: both columns of the pair are inside
+                    double r0 = accv[4 * j + 2 * i] * pow2i(esc + __ldg(P.Eb + n));
+                    double r1 = accv[4 * j + 2 * i + 1] * pow2i(esc + __ldg(P.Eb + n + 1));
+                    for (int s_ = 0; s_ < NS; s_++) {
+                        const double t0 = r0 + 6755399441055744.0, t1 = r1 + 6755399441055744.0;
+                        const double q0 = t0 - 6755399441055744.0, q1 = t1 - 6755399441055744.0;
+                        const unsigned short pk = (unsigned short)(((unsigned)__double2loint(t0) & 255u) | (((unsigned)__double2loint(t1) & 255u) << 8));
+                        *reinterpret_cast<unsigned short*>(dst0 + s_ * sstride + n) = pk;
+                        r0 = (r0 - q0) * 128.0; r1 = (r1 - q1) * 128.0;
                     }
                 }
-            } else if (P.accumulate) {
-                // partial result of this K range: fp64 reductions; every lane walks its own row, so the 32 reductions of one
-                // instruction go to 32 rows (scattered, but this epilogue runs once per 128 x 64 x K-range item)
-                if (mlane < P.M) {
-                    const int nb = nt * AR_BN;
-                    double* dst = P.C + off_lane + nb;
+                continue;
+            }
+            const long off = (P.inner > 0) ? (long)(m % P.inner) * P.ldc + (long)(m / P.inner) * P.N : (long)m * P.ldc;
+            double* dst = P.C + off;
+            if (P.accumulate) {
 #pragma unroll
-                    for (int j = 0; j < AR_BN; j++) {
-                        const int n = nb + j;
-                        if (n < P.N && (!P.symmetric || n >= mlane)) atomicAdd(dst + j, accv[j] * pow2i(ea_lane + __ldg(P.Eb + n)));
-                    }
-                }
-            } else if (mlane < P.M) {
-                const int nb = nt * AR_BN;
-                double* dst = P.C + off_lane + nb;
-                double vmax = 0.0;
-                if (((P.N | P.ldc) & 3) == 0 && nb + AR_BN <= P.N) {
-                    // every row segment starts on a 32-byte boundary: 256-bit stores, one full sector per lane and instruction
-                    // (scalar stores leave 32 eight-byte fragments per instruction for L2 to merge)
+                for (int j = 0; j < BN / 8; j++)
 #pragma unroll
-                    for (int j = 0; j < AR_BN; j += 4) {
-                        const int4 eb = __ldg(reinterpret_cast<const int4*>(P.Eb + nb + j));
-                        const double v0 = accv[j] * pow2i(ea_lane + eb.x), v1 = accv[j + 1] * pow2i(ea_lane + eb.y);
-                        const double v2 = accv[j + 2] * pow2i(ea_lane + eb.z), v3 = accv[j + 3] * pow2i(ea_lane + eb.w);
-                        asm volatile("st.global.v4.f64 [%0], {%1, %2, %3, %4};" ::"l"(dst + j), "d"(v0), "d"(v1), "d"(v2), "d"(v3) : "memory");
-                        vmax = fmax(fmax(vmax, fmax(fabs(v0), fabs(v1))), fmax(fabs(v2), fabs(v3)));
+                    for (int c = 0; c < 2; c++) {
+                        const int n = nb + 8 * j + cq + c;
+                        if (n < P.N && (!P.symmetric || n >= m)) atomicAdd(dst + n, accv[4 * j + 2 * i + c] * pow2i(ea + __ldg(P.Eb + n)));
                     }
+                continue;
+            }
+            double vmax = 0.0;
+#pragma unroll
+            for (int j = 0; j < BN / 8; j++) {
+                const int n = nb + 8 * j + cq;
+                if (n + 1 < P.N && ((off + n) & 1) == 0) {
+                    // both columns inside and 16-byte aligned: one 128-bit store
+                    const double v0 = accv[4 * j + 2 * i] * pow2i(ea + __ldg(P.Eb + n));
+                    const double v1 = accv[4 * j + 2 * i + 1] * pow2i(ea + __ldg(P.Eb + n + 1));
+                    *reinterpret_cast<double2*>(dst + n) = make_double2(v0, v1);
+                    vmax = fmax(vmax, fmax(fabs(v0), fabs(v1)));
                 } else {
 #pragma unroll
-                    for (int j = 0; j < AR_BN; j++)
-                        if (nb + j < P.N) { const double v = accv[j] * pow2i(ea_lane + __ldg(P.Eb + nb + j)); dst[j] = v; vmax = fmax(vmax, fabs(v)); }
+                    for (int c = 0; c < 2; c++)
+                        if (n + c < P.N) {
+                            const double v = accv[4 * j + 2 * i + c] * pow2i(ea + __ldg(P.Eb + n + c));
+                            dst[n + c] = v;
+                            vmax = fmax(vmax, fabs(v));
+                        }
                 }
-                if (P.rowmax && vmax > 0.0)
-                    atomicMax(P.rowmax + (P.inner > 0 ? mlane % P.inner : mlane), (unsigned long long)__double_as_longlong(vmax));
             }
-            if (stamp) P.dbg[it * 8 + 6] = clock64();   // tile stored
+            if (P.rowmax && vmax > 0.0)
+                atomicMax(P.rowmax + (P.inner > 0 ? m % P.inner : m), (unsigned long long)__double_as_longlong(vmax));
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
 // ---------------------------------------------------------------------------------------------- slicing kernels

@@ -1,4 +1,4 @@
-// i8gemm_host.hpp — host interface of the tcgen05 int8-slice GEMM (i8gemm.cu)
+// i8gemm_host.hpp — host interface of the int8-slice tensor-core GEMM (i8gemm.cu)
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -27,10 +27,7 @@ void gemm_ar(const SliceStack& A, int a_row0, int M, const SliceStack& B, double
              unsigned long long* rowmax = nullptr, const SliceStack* Yout = nullptr, int y_ncolp = 0);
 void split_rows_prepare(SliceStack& S, int rows, int k, int ns, cudaStream_t st);
 void split_rows_premax(SliceStack& S, const double* X, long ldx, int rows, int k, int ns, cudaStream_t st);
-// C[m*ldc + n] += A B^T on the A-stationary all-groups-resident kernel (stage 2 of DF-K); upper triangle only when symmetric
+// C[m*ldc + n] += A B^T (stage 2 of DF-K); upper triangle only when symmetric
 void gemm_ar_acc(const SliceStack& A, const SliceStack& B, double* C, long ldc, bool symmetric, cudaStream_t st);
-// C[m*ldc + n] (or the transposed scatter when inner>0, see GemmParams) += A B^T
-void gemm(const SliceStack& A, const SliceStack& B, double* C, long ldc, int inner, bool symmetric, cudaStream_t st,
-          long long* dbg = nullptr);
 }  // namespace i8g
 }  // namespace b200jk

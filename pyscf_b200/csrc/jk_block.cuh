@@ -52,8 +52,8 @@ constexpr int pow2ceil(int x) { int p = 1; while (p < x) p *= 2; return p; }
 //    once per part it holds (ncu: 20 of 32 threads active per instruction in (fd|dp)).
 //  * PPW (B2_PPW, classes with NP > 1 and NKL <= 32): a group is NP warps, warp w holds part w of QPG = 32 / NKL quartets,
 //    so no warp ever mixes parts.  Logical lane id inside a quartet stays g = part * NKL + (c,d).
-// classes that measured faster with the part-per-warp layout on B200 (benzene/cc-pVTZ, profiles/r02_ab_direct_variants.txt:
-// dd|pp -18 %, ff|ds -13 %, fd|ds -6 %, dd|dp, dd|ds, fd|pp -4..-6 %); (fd|dp), (ff|dp), (dd|ps) lose 10-35 % and stay as they were.
+// classes given the part-per-warp layout: chosen by A/B timing of benzene/cc-pVTZ on an earlier GPU generation, not re-measured
+// on the H100 (tools/build_variant.sh + tools/ab_direct.py repeat that A/B).
 // B2_PPW = 1 forces the layout for every class with NP > 1 (A/B builds), -1 switches it off everywhere.
 constexpr bool class_prefers_ppw(int li, int lj, int lk, int ll)
 {
@@ -409,8 +409,8 @@ void jk_block(const KParams& P, int bx, int by, BlockSmem<C>& sm)
 #endif
 
     // The CTA's ket range may be longer than the shared list: it is walked in sub-chunks of KCH_MAX kets (screen, compact,
-    // process), the stationary J[ij] block staying in registers across all of them.  Fewer, longer CTAs measured faster
-    // (profiles/r02_ab_direct_host_knobs.txt: the per-CTA prologue and the drain of the last batches are not free).
+    // process), the stationary J[ij] block staying in registers across all of them.  Fewer, longer CTAs amortise the per-CTA
+    // prologue and the drain of the last batches.
     for (int sub = kbeg; sub < kend; sub += KCH_MAX) {
         const int send = (sub + KCH_MAX < kend) ? sub + KCH_MAX : kend;
         if (sub > kbeg) {

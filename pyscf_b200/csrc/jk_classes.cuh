@@ -15,8 +15,7 @@ constexpr int lane_eff_permille(int g) { return g <= 32 ? (32 / g) * g * 1000 / 
 #define B2_NVMAX 30        // largest register block (doubles) of ERI accumulators per thread
 #endif
 #ifndef B2_WANT_CTAS
-#define B2_WANT_CTAS 2     // CTAs per SM a class launch aims for when it sizes the ket chunks (measured on B200, benzene/cc-pVTZ:
-                           // 64: 22.6 ms, 32: 21.5, 16: 19.8, 8: 18.4, 4: 17.6, 3: 17.4, 2: 17.2, 1: 17.4; B200JK_WANT_CTAS overrides at run time)
+#define B2_WANT_CTAS 2     // CTAs per SM a class launch aims for when it sizes the ket chunks (B200JK_WANT_CTAS overrides at run time)
 #endif
 #ifndef B2_PBMAX
 #define B2_PBMAX 1         // largest primitive batch (QClass::PB) of the block kernels; 1 = one primitive quartet per round
@@ -51,12 +50,30 @@ constexpr int choose_pb(int g, int nr, int h_bytes, int nslot)
     return pb;
 }
 
+// SMs of the current device, queried once per device (the CPU emulation models an H100 SXM: 132)
+inline long device_sm_count()
+{
+#ifndef B200JK_EMULATE
+    static int cache[64] = {0};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+    if (!cache[dev]) {
+        int n = 0;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+        cache[dev] = n;
+    }
+    return cache[dev];
+#else
+    return 132;
+#endif
+}
+
 // kets per CTA: at least one batch (`unit` kets in flight per CTA), at most `cap`, and small enough that
-// the class fills the 148 SMs several times over
+// the class fills the SMs several times over
 inline int pick_kchunk(int nbra, int nket, int unit, int cap)
 {
     static const long want_env = getenv("B200JK_WANT_CTAS") ? atol(getenv("B200JK_WANT_CTAS")) : 0;   // tuning experiment
-    long want_ctas = 148L * (want_env > 0 ? want_env : B2_WANT_CTAS);
+    long want_ctas = device_sm_count() * (want_env > 0 ? want_env : B2_WANT_CTAS);
     long ny = (want_ctas + nbra - 1) / nbra;
     long kc = (nket + ny - 1) / ny;
     if (kc < unit) kc = unit;
@@ -93,11 +110,11 @@ __global__ void __launch_bounds__(TpqCfg<C>::NT) jk_tpq_kernel(const KParams P)
     const int bx = blockIdx.x * P.shard_world + P.shard_rank;
     if (bx < P.nbra) tpq_block<C, SR>(P, bx, blockIdx.y, blockIdx.z);
 }
-// Register cap per class.  Most block kernels need 180-255 registers, i.e. ONE 192-thread CTA (6 warps) per SM; capping
-// them at 168 registers (two resident CTAs) wins 10-35 % on most classes and loses 15-40 % on the few whose working set
-// does not fit (spills): measured per class on B200, profiles/r01_ab_direct_variants.txt (column minb2).  The cap is applied
-// where it measured faster; the other kernels keep the plain bound (an explicit minBlocks = 1 is NOT equivalent: it makes
-// ptxas schedule seven classes 30-50 % slower).  B2_MINB = 0 / 2 forces one choice for every class (A/B builds).
+// Register cap per class: `__launch_bounds__(192, 2)` (<= 168 registers, two resident CTAs per SM) for most block kernels.
+// The exemptions below are an untuned carry-over, chosen by A/B timing on an earlier GPU generation and not re-timed on the
+// H100; for sm_90a, `-Xptxas -v` reports no spills in any capped kernel, and the exempted classes compile to <= 168
+// registers uncapped as well.  The other kernels keep the plain bound (an explicit minBlocks = 1 is NOT equivalent: it
+// changes ptxas's scheduling).  B2_MINB = 0 / 2 forces one choice for every class (A/B builds).
 #ifndef B2_MINB
 #define B2_MINB -1   // -1: per-class table below; 0: never cap; 2: cap every kernel of <= 192 threads
 #endif

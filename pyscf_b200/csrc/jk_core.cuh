@@ -1,4 +1,4 @@
-// jk_core.cuh — device-side arithmetic of the 4-center direct J/K path (sm_100a), written so that
+// jk_core.cuh — device-side arithmetic of the 4-center direct J/K path (sm_90a), written so that
 // the same templates also compile with g++ for the CPU SIMT-emulation tests (tests/emu).
 //
 // Replaces (reference file:line):
@@ -84,12 +84,10 @@ B2_HD void rys_root(const RysTables& tb, int n, int r, double x, double& u, doub
     const double* cp = tb.cheb + (size_t)RYS_NINT * RYS_ROW * (n * (n - 1) / 2) + (size_t)(iv * n + r) * RYS_ROW;
     double c[RYS_ROW];
 #if defined(__CUDA_ARCH__)
-    // one table row = 128 B = 4 x 256-bit loads (LDG.E.256 on sm_100a); rows are 32-byte aligned (b200jk_create)
+    // one table row = 128 B = 8 x 128-bit loads (the widest global load of sm_90); rows are 32-byte aligned (b200jk_create)
     B2_UNROLL
-    for (int j = 0; j < RYS_ROW / 4; j++)
-        asm volatile("ld.global.nc.v4.f64 {%0,%1,%2,%3}, [%4];"
-                     : "=d"(c[4 * j]), "=d"(c[4 * j + 1]), "=d"(c[4 * j + 2]), "=d"(c[4 * j + 3])
-                     : "l"(cp + 4 * j));
+    for (int j = 0; j < RYS_ROW / 2; j++)
+        asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(c[2 * j]), "=d"(c[2 * j + 1]) : "l"(cp + 2 * j));
 #else
     for (int j = 0; j < RYS_ROW; j++) c[j] = cp[j];
 #endif
@@ -113,13 +111,16 @@ struct PrimPair {  // 64 bytes, one per surviving primitive pair
     double PAx, PAy, PAz; // P - A   (A = centre of the first shell of the pair)
     double cc;            // sqrt(2 pi^(5/2)) * c_i c_j exp(-a_i a_j |AB|^2 / p) / p
 };
-// one PrimPair = 64 B = two 256-bit loads (a quarter of the L1 tag traffic of eight 64-bit loads)
+// one PrimPair = 64 B = four 128-bit loads (half the L1 tag traffic of eight 64-bit loads)
 B2_HD PrimPair load_prim(const PrimPair* p)
 {
 #if defined(__CUDA_ARCH__)
     PrimPair r;
-    asm volatile("ld.global.nc.v4.f64 {%0,%1,%2,%3}, [%4];" : "=d"(r.p), "=d"(r.Px), "=d"(r.Py), "=d"(r.Pz) : "l"(p));
-    asm volatile("ld.global.nc.v4.f64 {%0,%1,%2,%3}, [%4];" : "=d"(r.PAx), "=d"(r.PAy), "=d"(r.PAz), "=d"(r.cc) : "l"((const double*)p + 4));
+    const double* d = (const double*)p;
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(r.p), "=d"(r.Px) : "l"(d));
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(r.Py), "=d"(r.Pz) : "l"(d + 2));
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(r.PAx), "=d"(r.PAy) : "l"(d + 4));
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(r.PAz), "=d"(r.cc) : "l"(d + 6));
     return r;
 #else
     return *p;
@@ -136,15 +137,18 @@ struct ShellPair {  // 64 bytes
     int32_t pad;
 };
 
-static_assert(sizeof(ShellPair) == 64, "ShellPair is loaded as two 256-bit words");
-// one ShellPair = 64 B = two 256-bit loads
+static_assert(sizeof(ShellPair) == 64, "ShellPair is loaded as four 128-bit words");
+// one ShellPair = 64 B = four 128-bit loads
 B2_HD ShellPair load_pair(const ShellPair* p)
 {
 #if defined(__CUDA_ARCH__)
     ShellPair r;
     unsigned long long w0, w1, w2, w3;
-    asm volatile("ld.global.nc.v4.f64 {%0,%1,%2,%3}, [%4];" : "=d"(r.ABx), "=d"(r.ABy), "=d"(r.ABz), "=d"(r.q) : "l"(p));
-    asm volatile("ld.global.nc.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(w0), "=l"(w1), "=l"(w2), "=l"(w3) : "l"((const char*)p + 32));
+    const double* d = (const double*)p;
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(r.ABx), "=d"(r.ABy) : "l"(d));
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(r.ABz), "=d"(r.q) : "l"(d + 2));
+    asm volatile("ld.global.nc.v2.u64 {%0,%1}, [%2];" : "=l"(w0), "=l"(w1) : "l"(d + 4));
+    asm volatile("ld.global.nc.v2.u64 {%0,%1}, [%2];" : "=l"(w2), "=l"(w3) : "l"(d + 6));
     r.ish = (int32_t)(w0 & 0xffffffffu); r.jsh = (int32_t)(w0 >> 32);
     r.i0 = (int32_t)(w1 & 0xffffffffu); r.j0 = (int32_t)(w1 >> 32);
     r.prim_off = (int32_t)(w2 & 0xffffffffu); r.nprim = (int32_t)(w2 >> 32);

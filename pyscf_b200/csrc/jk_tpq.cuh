@@ -22,7 +22,7 @@ namespace b200jk {
 #ifndef B2_TPQ_KOUTER
 #define B2_TPQ_KOUTER 1      // 1: ket primitive loop outside the bra primitive loop (each thread loads its own ket primitive once
 #endif                       //    per ket primitive instead of once per primitive QUARTET; the bra primitive is warp-uniform).
-                             //    Measured on B200 (profiles/r02_ab_direct_variants.txt): ps|ss -19 %, ss|ss -27 %, no class slower.
+                             //    Chosen by A/B timing on an earlier GPU generation; not re-measured on the H100.
 #ifndef B2_TPQ_KCHUNK
 #define B2_TPQ_KCHUNK 512    // ket pairs examined per CTA (upper bound)
 #endif

@@ -1,4 +1,4 @@
-"""Density-fitted J/K on B200 behind the reference's `with_df` surface.
+"""Density-fitted J/K on H100 behind the reference's `with_df` surface.
 
 Mirrors (names, argument meaning, shapes):
   * df.DF(mol, auxbasis): build(), reset(), get_naoaux(), loop(), get_jk(dm, hermi, with_j, with_k,
@@ -98,7 +98,8 @@ class DF:
         return path
 
     def set_k_engine(self, engine='tcgen05', nslices=7):
-        """'tcgen05' (int8-slice tensor-core GEMMs, default) or 'dgemm' (cuBLAS FP64 yardstick)."""
+        """'tcgen05' (the engine's historical name: int8-slice GEMMs on the tensor cores, wgmma; default) or 'dgemm'
+        (cuBLAS FP64 yardstick)."""
         self.k_engine, self.k_slices = engine, nslices
         if self._handle is not None:
             h = self._handle
@@ -360,7 +361,7 @@ class _DFHF:
         return vj, vk
 
     def _exact_get_jk(self, mol, dm, hermi, with_j, with_k, omega):
-        """super().get_jk of the reference: the B200 4-center builder when jk.patch() was applied to the object before (its
+        """super().get_jk of the reference: the GPU 4-center builder when jk.patch() was applied to the object before (its
         instance override is kept as _b200_direct_jk), else the mean-field class's own get_jk."""
         f = getattr(self, '_b200_direct_jk', None)
         if f is not None:
@@ -369,7 +370,7 @@ class _DFHF:
 
 
 def density_fit(mf, auxbasis=None, with_df=None, only_dfj=False, device=0):
-    """df_jk.density_fit (pyscf/df/df_jk.py:31-102) with a B200 DF object: returns an object of the dynamic class
+    """df_jk.density_fit (pyscf/df/df_jk.py:31-102) with a GPU DF object: returns an object of the dynamic class
     (_DFHF, mf.__class__) sharing mf's attributes, whose get_jk is served by with_df.get_jk (J and K from the fitted tensor) or,
     with only_dfj=True, J from the tensor and K from the exact 4-center path (RIJONX, df_jk.py:157-179).  An object that is
     already density-fitted just gets the new with_df / only_dfj (df_jk.py:88-99)."""

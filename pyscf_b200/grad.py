@@ -1,4 +1,4 @@
-"""Nuclear-gradient J/K on B200: the role of pyscf.grad.rhf.get_jk / get_j / get_k (pyscf/grad/rhf.py:191-235)
+"""Nuclear-gradient J/K on H100: the role of pyscf.grad.rhf.get_jk / get_j / get_k (pyscf/grad/rhf.py:191-235)
 
     vj[x, i, j] = - sum_kl (nabla_x i  j | k l) D_lk            vk[x, i, l] = - sum_jk (nabla_x i  j | k l) D_jk
 

@@ -1,4 +1,4 @@
-"""Direct-SCF J/K on B200 behind the reference's plugin surface.
+"""Direct-SCF J/K on H100 behind the reference's plugin surface.
 
 Mirrors (same names, argument meaning, shapes and error behaviour):
   * scf.hf.get_jk(mol, dm, hermi, vhfopt, with_j, with_k, omega)      pyscf/scf/hf.py:963-1034
@@ -198,7 +198,7 @@ def get_jk(mol, dm, hermi=1, vhfopt=None, with_j=True, with_k=True, omega=None):
 
 
 def patch(mf, device=0, libpath=None):
-    """Install the B200 builder as `mf.get_jk` on a PySCF SCF object (instance override).
+    """Install the GPU builder as `mf.get_jk` on a PySCF SCF object (instance override).
 
     Keeps the reference semantics of SCF.get_jk (pyscf/scf/hf.py:2136-2160): one cached optimizer per omega (mf._opt there,
     mf._b200_opts here), dropped by mf.reset() (pyscf/scf/hf.py:2331: reset clears _opt) and rebuilt when the molecule's

@@ -1,4 +1,4 @@
-"""`get_veff` on top of the B200 J/K builders: the callers one level above `get_jk` on the hot path.
+"""`get_veff` on top of the GPU J/K builders: the callers one level above `get_jk` on the hot path.
 
 Mirrors (argument meaning, incremental-Fock behaviour, the `ecoul` / `vj` / `vk` tags the SCF loop reads back):
   * scf.hf.SCF.get_veff      pyscf/scf/hf.py:2172-2201   vhf = J - K/2, built from D - D_last when direct_scf

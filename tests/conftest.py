@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run with -m gpu on the B200 box)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run with -m gpu on an H100)')
 
 
 from pyscf_b200.gto.mole import geometry

@@ -275,7 +275,7 @@ def test_df_gpu_benzene_properties():
     st = d.stage_times()
     assert all(st[k][1] >= 1 and st[k][0] > 0 for k in ('j_rho', 'j_acc', 'k_gemm1', 'k_slice', 'k_gemm2')), st
     assert sum(v[0] for v in st.values()) <= d.stats()['ms_kernels'] * 1.05
-    assert abs(vk - d.get_jk(2 * c.dot(c.T))[1]).max() < 1e-9      # tcgen05 slices == FP64 general-density path
+    assert abs(vk - d.get_jk(2 * c.dot(c.T))[1]).max() < 1e-9      # int8 slices == FP64 general-density path
 
 
 @pytest.mark.gpu
@@ -297,7 +297,7 @@ def test_df_golden_vectors(name, geom, basis):
     dms = np.random.random((2, nao, nao))
     vj, vk = d.get_jk(dms, hermi=0)
     assert abs(vj - g['vj']).max() < 1e-9 and abs(vk - g['vk']).max() < 1e-9
-    # occupied-orbital path through both K engines (tcgen05 int8 slices, cuBLAS DGEMM)
+    # occupied-orbital path through both K engines (int8 slices on the tensor cores, cuBLAS DGEMM)
     c = np.linalg.qr(np.random.random((nao, 21)))[0]
     occ = np.full(21, 2.0)
     dm = TaggedDM((c * occ).dot(c.T), mo_coeff=c, mo_occ=occ)
@@ -305,3 +305,27 @@ def test_df_golden_vectors(name, geom, basis):
     k_dg = d.set_k_engine('dgemm').get_jk(dm, with_j=False)[1]
     k_gen = d.get_jk(np.asarray(dm), hermi=1, with_j=False)[1]
     assert abs(k_tc - k_dg).max() < 1e-10 and abs(k_tc - k_gen).max() < 1e-10
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('M,N,K,ns,sym', [(300, 77, 333, 7, 0), (65, 33, 129, 7, 0), (1, 200, 40, 7, 0), (257, 257, 130, 7, 1),
+                                          (140, 95, 300, 3, 0), (129, 129, 256, 2, 1), (70, 45, 128, 8, 0), (33, 31, 17, 1, 0)])
+def test_i8gemm_against_numpy(M, N, K, ns, sym):
+    """The int8-slice tensor-core GEMM itself (b200jk_i8gemm_test: slicing + i8gemm_kernel, accumulate mode): C = A B^T with
+    partial 128 x 32 tiles, K not a multiple of 128, 1..8 slices, and the upper-triangle-only symmetric mode (B = A)."""
+    from pyscf_b200 import lib
+    mol = gto.M(atom=H2O, basis='sto-3g')
+    h = lib.Handle(mol._atm, mol._bas, np.array(mol._env, dtype=np.float64))
+    rng = np.random.RandomState(M * 7 + N + ns)
+    A = rng.standard_normal((M, K)) * np.exp(rng.uniform(-6, 6, (M, 1)))    # rows of very different magnitude
+    B = A.copy() if sym else rng.standard_normal((N, K)) * np.exp(rng.uniform(-6, 6, (N, 1)))
+    C = np.zeros((M, N))
+    h.check(h.lib.b200jk_i8gemm_test(h._h, M, N, K, lib.dptr(A), lib.dptr(B), lib.dptr(C), ns, sym), 'b200jk_i8gemm_test')
+    ref = A.dot(B.T)
+    if sym:
+        ref = np.triu(ref)
+    # slicing error: every row to 2^-(6+7(ns-1)) of its largest element, pairs k + l >= ns dropped
+    scale = abs(A).max(1)[:, None] * abs(B).max(1)[None, :] * K
+    err = abs(C - ref) / scale
+    assert err.max() < 2.0 ** (-(7 * ns - 3)), (err.max(), 2.0 ** (-(7 * ns - 3)))
+    h.close()

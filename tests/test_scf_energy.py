@@ -1,4 +1,4 @@
-"""Converged SCF energies through the B200 J/K builders equal the reference's published values
+"""Converged SCF energies through the GPU J/K builders equal the reference's published values
 (north_star: "converged SCF energy identical to reference tolerance").
   RHF  H2O/cc-pVDZ            -76.026765673119627   pyscf/scf/test/test_rhf.py:371-372
   DF-RHF H2O/cc-pVDZ/weigend  -76.025936299702536   pyscf/df/test/test_df_jk.py:57-59

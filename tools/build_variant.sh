@@ -12,7 +12,7 @@ cp $ROOT/pyscf_b200/csrc/*.cu $ROOT/pyscf_b200/csrc/*.cuh $ROOT/pyscf_b200/csrc/
 cp $ROOT/include/b200jk.h $SRC/include/
 mkdir -p $SRC/csrc/../../include && cp $ROOT/include/b200jk.h $SRC/csrc/../../include/ 2>/dev/null || true
 if [ $# -gt 1 ]; then REV=$1; shift; for f in "$@"; do git -C $ROOT show $REV:pyscf_b200/csrc/$f > $SRC/csrc/$f; done; fi
-NV="nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 --expt-relaxed-constexpr -Xcompiler -fPIC -Xptxas -v -I$ROOT/include $FLAGS"
+NV="nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 --expt-relaxed-constexpr -Xcompiler -fPIC -Xptxas -v -I$ROOT/include $FLAGS"
 cd $SRC/csrc
 for i in 0 1 2 3 4 5 6 7 8 9; do
   ( $NV -DB2_BRA_ID=$i -c jk_class_tu.cu -o $SRC/obj/jk_bra_$i.o 2> $SRC/obj/ptxas_$i.log || { cat $SRC/obj/ptxas_$i.log; exit 1; } ) &

@@ -12,9 +12,9 @@ column, and J/K of a density SUPPORTED ON A FEW SHELLS S only need the slab (P|s
     contraction lengths of both GEMM stages are the real ones), D_S = C_S C_S^T:
         K[i,l]  = sum_P sum_{j,k in S} B[P,i,j] D_S[j,k] B[P,k,l]     every element of K, from the slab alone
         J[s,nu] = sum_P B[P,s,nu] rho_P,  rho_P = sum_{j,k in S} B[P,j,k] D_S[j,k]    the rows s in S of J
-    stored as `vk_idx`/`vk_val` (sampled elements), fp(K), and the J rows.  Both K engines (tcgen05 int8 slices on the
+    stored as `vk_idx`/`vk_val` (sampled elements), fp(K), and the J rows.  Both K engines (int8 slices on the
     orbital tag, FP64 general path on the bare matrix) are compared with these on the GPU (tests/test_df_size.py, bench.py).
-Usage: python tools/make_golden_df_size.py [c60 taxol gly30 gly30_lr]
+Usage: python tools/make_golden_df_size.py [c60 taxol taxol_svp gly30 gly30_lr]
 """
 import os
 import sys
@@ -31,10 +31,14 @@ from oracle import oracle as O   # noqa: E402
 CASES = {   # name: (geometry, basis, nocc, omega)
     'c60': ('c60', 'def2-svp', 180, None),
     'taxol': ('taxol', 'def2-tzvp', 226, None),
+    # one GPU of 80 GB holds its 28 GB tensor but not the int8 slices of all its rows: resident and re-cut slices both run
+    'taxol_svp': ('taxol', 'def2-svp', 226, None),
     'gly30': ('gly30', 'cc-pvdz', 455, None),
     'gly30_lr': ('gly30', 'cc-pvdz', 455, 0.3),
     'gly4': ('gly4', 'cc-pvdz', 65, None),          # small: the same fixture at a size the CPU tests can build in full
 }
+# fixtures kept below 1 MB: one shell pair per angular-momentum pair type, two components each, fewer sampled K elements
+SMALL = {'taxol_svp'}
 
 
 def slab_coeff(nao, nocc, sao, seed=7):
@@ -123,7 +127,8 @@ def main(name):
         def solve(x):
             return winv.dot(x)
     # ---- sampled columns
-    pairs = pick_pairs(mol, rng)
+    small = name in SMALL
+    pairs = pick_pairs(mol, rng, per_type=1 if small else 2)
     t0 = time.time()
     j3c, col0 = O.int3c2e_pairs(mol, auxmol, pairs)
     cd = solve(j3c)
@@ -131,7 +136,7 @@ def main(name):
     for p, (i, j) in enumerate(pairs):
         di, dj = loc[i + 1] - loc[i], loc[j + 1] - loc[j]
         comps = [(a, b) for a in range(di) for b in range(dj) if loc[i] + a >= loc[j] + b]
-        for idx in rng.choice(len(comps), size=min(3, len(comps)), replace=False):
+        for idx in rng.choice(len(comps), size=min(2 if small else 3, len(comps)), replace=False):
             a, b = comps[idx]
             mu, nu = loc[i] + a, loc[j] + b
             cols.append(mu * (mu + 1) // 2 + nu)
@@ -171,7 +176,7 @@ def main(name):
         t = np.matmul(d_ss, b)                                 # D_SS B_P[S,:]   [pb, ns, nao]
         vk += b.reshape(-1, nao).T.dot(t.reshape(-1, nao))     # sum_{P,s} B[P,s,i] T[P,s,n]  (BLAS)
     print('  J rows / K from the slab %.1f s; |K|max %.3g |J|max %.3g' % (time.time() - t0, abs(vk).max(), abs(vj_rows).max()), flush=True)
-    nsamp = 6000
+    nsamp = 3000 if small else 6000
     ii, ll = rng.randint(nao, size=nsamp), rng.randint(nao, size=nsamp)
     ii[:len(sao)] = sao
     ll[:len(sao)] = sao[::-1]

@@ -8,7 +8,7 @@ def parse(pattern):
     out = {}
     for f in glob.glob(pattern):
         txt = open(f).read()
-        for m in re.finditer(r"Compiling entry function '(\S+)' for 'sm_100a'.*?(\d+) bytes stack frame, (\d+) bytes spill stores.*?Used (\d+) registers", txt, re.S):
+        for m in re.finditer(r"Compiling entry function '(\S+)' for 'sm_90a'.*?(\d+) bytes stack frame, (\d+) bytes spill stores.*?Used (\d+) registers", txt, re.S):
             mm = re.search(r'jk_(class_kernel_2cta|class_kernel|tpq_kernel)INS_6QClassILi(\d)ELi(\d)ELi(\d)ELi(\d)ELi(\d+)E(?:Li(\d+)E)?EELb(\d)', m.group(1))
             if mm and mm.group(8) == '0':
                 key = '(%s%s|%s%s)' % tuple('spdfg'[int(x)] for x in mm.group(2, 3, 4, 5))

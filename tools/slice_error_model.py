@@ -3,7 +3,7 @@
 
 Mirrors i8gemm.cuh: every row x is scaled by 2^(6-e) (|x| 2^(6-e) < 64, e from frexp of the row maximum) and cut into signed
 slices q_s = rint(r_s), r_{s+1} = 128 (r_s - q_s); the product keeps the slice pairs with k + l < ns, each accumulated
-exactly (int32 in TMEM, int64 here) and weighted 2^(ea + eb - 12 - 7 (k + l)).  Prints max |C_sliced - C| / max |C| for
+exactly (int32 registers on the GPU, int64 here) and weighted 2^(ea + eb - 12 - 7 (k + l)).  Prints max |C_sliced - C| / max |C| for
 random rows with a chosen dynamic range, for a contraction length K — the quantity behind "7 slices -> 4e-13 on C60" and the
 question whether 6 slices would still meet the 1e-9 bar (DESIGN.md §7 item 2a).
 usage: python tools/slice_error_model.py [K=65536] [rows=24] [decades=6]"""
