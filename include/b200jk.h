@@ -148,9 +148,34 @@ int b200jk_fp64_peak(b200jk_handle h, double* tflops);
  * ms[100]: entry [cb*10+ck], pair class id = l1*(l1+1)/2+l2 (ss,ps,pp,ds,dp,dd,fs,fp,fd,ff). */
 int b200jk_set_profile(b200jk_handle h, int on);
 int b200jk_get_class_times(b200jk_handle h, double* ms, int n);
-/* Self-test of the int8-slice tensor-core GEMM used by DF-K: C[M,N] = A[M,K] B[N,K]^T with `ns` 7-bit slices. */
+/* Caps on the blocking of the int8-slice K build (tests): at most max_block_rows auxiliary rows per K block and at most
+ * max_resident_rows packed rows whose slices stay resident between calls (the rest are re-cut per block); -1 keeps the
+ * automatic choice, which a cap can only shrink. */
+int b200jk_df_set_kblock(b200jk_handle h, int max_block_rows, int max_resident_rows);
+/* Self-test of the int8-slice tensor-core GEMM used by DF-K: C[M,N] = A[M,K] B[N,K]^T with `ns` 7-bit slices (split_rows +
+ * gemm_ar_acc with automatic K ranges; upper triangle only when symmetric).  b200jk_i8engine_test with stage 2. */
 int b200jk_i8gemm_test(b200jk_handle h, int M, int N, int K, const double* A, const double* B, double* C, int ns,
                        int symmetric);
+/* Self-test of the int8-slice engine of DF-K (i8gemm.cuh) on host buffers, `ns` 7-bit slices.  Every output may be NULL.
+ * Operand A: packed = 0: a[ra][k], sliced by split_rows (the long-row kernels when k >= 8192 and ra < 4096) or, with
+ *   a_rowmax[ra] (row maxima, >= 0), by split_rows_premax; packed = 1: ra packed tensor rows a[ra][k(k+1)/2] (nao = k),
+ *   packed_rowexp into rowexp / rownorm2 [ra][k], then split_packed into the ra*k unpacked rows (P, a).
+ * Stacks come back whole, pads included: q[ns][Rp][Kp] int8 and E[Rp] (Rp = rows rounded up to 256, Kp = k rounded up to 128).
+ * stage 0: slicing only.  stage 1: b[rb][k] sliced by split_rows; gemm_ar on rows [a_row0, a_row0 + m) of A with the transposed
+ *   scatter `inner` (0: none) into c ([inner][ceil(m/inner) rb], else [m][rb]) and the row maxima into rowmax ([inner] or [m],
+ *   0 where none); with y_ncolp > 0 (packed A, inner = k) it writes the Y slices instead: qy / ey, Y stack of k rows and
+ *   (m/k) y_ncolp columns, exponent bounds from the row norms of the block and the column norms of b.
+ * stage 2: c[ra][rb] = A B^T by gemm_ar_acc from zero, upper triangle only when symmetric; kb_per > 0 forces K ranges of
+ *   kb_per blocks of 128. */
+typedef struct {
+    int stage, packed, ns;
+    const double* a; int ra, k; const double* a_rowmax;
+    const double* b; int rb;
+    int a_row0, m, inner, y_ncolp, symmetric, kb_per;
+    int8_t* qa; int32_t* ea; int8_t* qb; int32_t* eb; int32_t* rowexp; float* rownorm2;
+    double* c; double* rowmax; int8_t* qy; int32_t* ey;
+} b200jk_i8test;
+int b200jk_i8engine_test(b200jk_handle h, b200jk_i8test* t);
 int b200jk_get_stats(b200jk_handle h, b200jk_stats* out);
 const char* b200jk_last_error(b200jk_handle h);
 const char* b200jk_version(void);

@@ -63,6 +63,7 @@ struct DFState {
     size_t ws_rows = 0, ws_nocc = 0, ws_ndm = 0, ws_occ_ndm = 0;
     int k_mode = 1;      // 0: cuBLAS DGEMM (FP64 pipe), 1: int8 slices on the tensor cores (i8gemm.cuh)
     int k_slices = 7;
+    int kb_max = -1, np_max = -1;   // b200jk_df_set_kblock: caps on the rows per K block / resident packed rows (-1: none)
     double* d_Y2 = nullptr; double* d_occT = nullptr; size_t y2_cap = 0, occT_cap = 0;
 #ifndef B200JK_EMULATE
     cublasHandle_t cublas = nullptr;
@@ -934,6 +935,7 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
         // rows per block: the block is read twice (rho, then J) and should stay in L2; K unpacks it to nao^2
         int rb = (int)std::max<long>(1, std::min<long>(naux, (40L << 20) / (npair * 8)));
         int kb = (int)std::max<long>(1, std::min<long>(naux, (2048L << 20) / (n2 * 8)));
+        if (d->kb_max > 0) kb = std::min(kb, d->kb_max);
         if ((size_t)n_dm > d->ws_ndm) {
             for (double** p : {&d->d_dmtril, &d->d_rho, &d->d_vjtril, &d->d_dm, &d->d_vk, &d->d_vj}) { dev_free(*p); *p = nullptr; }
             d->d_dmtril = (double*)dev_alloc((size_t)n_dm * npair * 8);
@@ -1033,11 +1035,10 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
             const bool tc = d->k_mode == 1;
             const bool k_sym = use_occ || hermi == 1;   // the result is symmetric: compute the upper triangle, mirror at the end
             if (tc) {
-                // int32 accumulation bound: pairs(<=ns) * K * 64*64 < 2^31
-                int kmax = (int)((1L << 19) / d->k_slices);
+                // stage 2 in one K range: pairs(<=ns) * K * 64*64 <= 2^31 - 1 (gemm_ar_acc splits K further where this does not
+                // hold; gemm_ar rejects a stage 1 whose nao breaks the bound)
+                int kmax = (int)(((1L << 31) - 1) / (4096L * d->k_slices));
                 kb = std::max(1, std::min(kb, kmax / ((ncol + 15) & ~15)));   // stage 2 contracts over (P, i) with i padded to 16
-                // stage 1 contracts over nao with tensor digits up to 127 (split_packed_kernel) against balanced digits (<= 64)
-                if ((long)nao * d->k_slices * 127 * 64 >= (1L << 31)) throw std::runtime_error("nao too large for the int32 accumulators of DF-K stage 1");
                 if ((size_t)kb * ncol * nao > d->y2_cap) { dev_free(d->d_Y2); d->y2_cap = (size_t)kb * ncol * nao; d->d_Y2 = (double*)dev_alloc(d->y2_cap * 8); }
                 if ((size_t)ncol * nao > d->occT_cap) { dev_free(d->d_occT); d->occT_cap = (size_t)ncol * nao; d->d_occT = (double*)dev_alloc(d->occT_cap * 8); }
                 if (!d->d_rowexp) {
@@ -1063,6 +1064,7 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
                 if (freeb * 0.85 > (double)reserve) np = (long)((freeb * 0.85 - (double)reserve) / (double)per_row);
                 if (np >= nloc) np = nloc;
                 else if (np < nloc / 10) np = 0;                      // not worth a second code path
+                if (d->np_max >= 0) np = std::min(np, (long)d->np_max);
                 while (np > 0 && (size_t)np * nao >= (1UL << 31) - 256) np--;   // row index of the stack is an int
                 d->sa_np = (int)np;
                 if (np > 0) {
@@ -1277,6 +1279,17 @@ extern "C" int b200jk_df_stage_times(b200jk_handle h, double* ms, int* count, in
         ms[i] = i < B200JK_DF_NSTAGE ? h->df->stage_ms[i] : 0.0;
         count[i] = i < B200JK_DF_NSTAGE ? h->df->stage_n[i] : 0;
     }
+    return 0;
+}
+
+extern "C" int b200jk_df_set_kblock(b200jk_handle h, int max_block_rows, int max_resident_rows)
+{
+    if (!h || !h->df) { set_err(h, "call b200jk_df_build first"); return 1; }
+    if (max_block_rows == 0 || max_block_rows < -1 || max_resident_rows < -1) { set_err(h, "bad block / resident row cap"); return 1; }
+    h->df->kb_max = max_block_rows; h->df->np_max = max_resident_rows;
+#ifndef B200JK_EMULATE
+    h->df->sa_decided = false;     // the resident stack is re-cut on the next K build
+#endif
     return 0;
 }
 

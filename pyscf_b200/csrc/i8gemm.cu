@@ -59,6 +59,7 @@ void split_rows_prepare(SliceStack& S, int rows, int k, int ns, cudaStream_t st)
 {
     S.alloc(rows, k, ns);
     S.zeroed_for = 0;
+    S.dmax = 64;
     CK(cudaMemsetAsync(S.maxbits, 0, (size_t)rows * 8, st));
 }
 void split_rows_premax(SliceStack& S, const double* X, long ldx, int rows, int k, int ns, cudaStream_t st)
@@ -79,6 +80,7 @@ void split_rows(SliceStack& S, const double* X, long ldx, int rows, int k, int n
 {
     S.alloc(rows, k, ns);
     S.zeroed_for = 0;
+    S.dmax = 64;
     if (S.Rp > rows) {   // zero the pad rows of every slice
         for (int s = 0; s < ns; s++)
             CK(cudaMemsetAsync(S.q + ((size_t)s * S.Rp + rows) * S.Kp, 0, (size_t)(S.Rp - rows) * S.Kp, st));
@@ -126,6 +128,7 @@ void y_prepare(SliceStack& S, int nao, int nr, int ncolp, int ns, const float* r
 {
     const int k = nr * ncolp;
     S.alloc(nao, k, ns);
+    S.dmax = 64;
     const bool same = (S.zeroed_for == (long)nao * 1000003L + k);
     if (!same) {
         CK(cudaMemsetAsync(S.q, 0, (size_t)ns * S.Rp * S.Kp, st));
@@ -139,6 +142,7 @@ void y_prepare(SliceStack& S, int nao, int nr, int ncolp, int ns, const float* r
 void split_packed_into(SliceStack& S, int out_row0, const double* cderi, long npair, int nao, int nr, const int* rowexp, cudaStream_t st)
 {
     if (S.K != nao) throw std::runtime_error("split_packed: stack width does not match nao");
+    S.dmax = S.ns <= 7 ? 127 : 64;
     const unsigned nt = (unsigned)(S.Kp / PT);
     for (int p0 = 0; p0 < nr; p0 += 32768) {
         int n = std::min(32768, nr - p0);
@@ -202,12 +206,24 @@ static void launch(unsigned grid, const CUtensorMap& ta, const CUtensorMap& tb, 
     CK(cudaGetLastError());
 }
 
+// Longest K range (in K blocks) whose slice-pair group sums are exact in int32: group ns-1 adds ns pairs of kr products of at
+// most dmax_A dmax_B each, so ns kr dmax_A dmax_B <= 2^31 - 1.  Columns at or past the shorter operand's K are zero and count
+// for nothing.  Returns the number of K blocks of the whole product when it fits in one range.
+static int int32_kblocks(const SliceStack& A, const SliceStack& B)
+{
+    const long kmax = ((1L << 31) - 1) / ((long)A.ns * A.dmax * B.dmax);
+    if (std::min(A.K, B.K) <= kmax) return A.Kp / BK;
+    return (int)(kmax / BK);
+}
+
 // stage-1 GEMM of DF-K: rows [a_row0, a_row0+M) of A times B^T, one work item per tile, persistent grid
 void gemm_ar(const SliceStack& A, int a_row0, int M, const SliceStack& B, double* C, long ldc, int inner, cudaStream_t st,
              unsigned long long* rowmax, const SliceStack* Yout, int y_ncolp)
 {
     if (A.Kp != B.Kp || A.ns != B.ns) throw std::runtime_error("i8gemm_ar: operand stacks disagree");
     if (A.ns < 1 || A.ns > MAXS) throw std::runtime_error("i8gemm_ar: slice count out of range");
+    if (a_row0 < 0 || M < 0 || a_row0 + M > A.R) throw std::runtime_error("i8gemm_ar: row block outside the A stack");
+    if (int32_kblocks(A, B) < A.Kp / BK) throw std::runtime_error("i8gemm_ar: K too long for exact int32 slice-pair sums");
     const int nsm = sm_count();
     CUtensorMap ta, tb;
     make_tmap(&ta, A.q, (uint64_t)A.ns * A.Rp, A.Kp, BM);
@@ -227,7 +243,7 @@ void gemm_ar(const SliceStack& A, int a_row0, int M, const SliceStack& B, double
 
 // C += A B^T (upper triangle only when symmetric): stage 2 of DF-K.  Work items = tiles x K ranges, sized to fill whole
 // waves of the persistent grid.
-void gemm_ar_acc(const SliceStack& A, const SliceStack& B, double* C, long ldc, bool symmetric, cudaStream_t st)
+void gemm_ar_acc(const SliceStack& A, const SliceStack& B, double* C, long ldc, bool symmetric, cudaStream_t st, int kb_per)
 {
     if (A.Kp != B.Kp || A.ns != B.ns) throw std::runtime_error("i8gemm_ar_acc: operand stacks disagree");
     if (A.ns < 1 || A.ns > MAXS) throw std::runtime_error("i8gemm_ar_acc: slice count out of range");
@@ -243,16 +259,24 @@ void gemm_ar_acc(const SliceStack& A, const SliceStack& B, double* C, long ldc, 
     for (int mt = 0; mt < ntm; mt++) tiles += symmetric ? std::max(0, ntn - (BM / BN) * mt) : ntn;
     if (symmetric && ntn < (BM / BN) * (ntm - 1) + 1) throw std::runtime_error("i8gemm_ar_acc: symmetric product needs a square output");
     const int nkb = A.Kp / BK;
-    // K ranges: >= 8 K blocks each; among those the count that wastes the least of the last wave of the persistent grid
-    int best = 1; double best_eff = -1.0;
-    for (int ks = 1; ks <= std::max(1, nkb / 8); ks++) {
-        const int per = (nkb + ks - 1) / ks, kse = (nkb + per - 1) / per;
-        const long items = (long)tiles * kse;
-        const double eff = (double)items / ((double)nsm * ((items + nsm - 1) / nsm));
-        if (eff > best_eff + 1e-9) { best_eff = eff; best = kse; }
-        if (items > 12L * nsm) break;
+    const int kb_lim = int32_kblocks(A, B);
+    if (kb_lim < 1) throw std::runtime_error("i8gemm_ar_acc: slice count too large for exact int32 slice-pair sums");
+    if (kb_per > kb_lim) throw std::runtime_error("i8gemm_ar_acc: K range too long for exact int32 slice-pair sums");
+    if (kb_per > 0) {
+        P.kb_per = std::min(kb_per, nkb);
+    } else {
+        // K ranges: >= 8 K blocks each; among those the count that wastes the least of the last wave of the persistent grid
+        const int ks_min = (nkb + kb_lim - 1) / kb_lim;
+        int best = ks_min; double best_eff = -1.0;
+        for (int ks = ks_min; ks <= std::max(ks_min, nkb / 8); ks++) {
+            const int per = (nkb + ks - 1) / ks, kse = (nkb + per - 1) / per;
+            const long items = (long)tiles * kse;
+            const double eff = (double)items / ((double)nsm * ((items + nsm - 1) / nsm));
+            if (eff > best_eff + 1e-9) { best_eff = eff; best = kse; }
+            if (items > 12L * nsm) break;
+        }
+        P.kb_per = (nkb + best - 1) / best;
     }
-    P.kb_per = (nkb + best - 1) / best;
     P.ksplit = (nkb + P.kb_per - 1) / P.kb_per;
     P.ntiles = tiles;
     const long items = (long)tiles * P.ksplit;
@@ -263,42 +287,96 @@ void gemm_ar_acc(const SliceStack& A, const SliceStack& B, double* C, long ldc, 
 }  // namespace b200jk
 #endif
 
+// Self-test of the int8-slice engine on host buffers (include/b200jk.h): slicing kernels, stage-1 and stage-2 GEMM, outputs
+// copied back whole (pads included) so that tests can compare them bit for bit with a model of the engine.
+extern "C" int b200jk_i8engine_test(b200jk_handle h, b200jk_i8test* t)
+{
+    if (!h) return 1;
+    if (!t) { set_err(h, "b200jk_i8engine_test: no arguments"); return 1; }
+#ifndef B200JK_EMULATE
+    std::vector<void*> tmp;
+    auto alloc = [&](size_t n) { void* p = dev_alloc(n); tmp.push_back(p); return p; };
+    b200jk::i8g::SliceStack SA, SB, SY;
+    int rc = 0;
+    try {
+        using namespace b200jk::i8g;
+        const int ns = t->ns, k = t->k, ra = t->ra, rb = t->rb;
+        if (ns < 1 || ns > MAXS) throw std::runtime_error("ns out of range");
+        if (!t->a || ra < 1 || k < 1 || t->stage < 0 || t->stage > 2) throw std::runtime_error("bad operand A or stage");
+        if (t->stage > 0 && (!t->b || rb < 1)) throw std::runtime_error("bad operand B");
+        CK(cudaSetDevice(h->device));
+        cudaStream_t st = h->stream;
+        float* d_norm2 = nullptr;
+        if (t->packed) {
+            const long npair = (long)k * (k + 1) / 2;
+            double* dA = (double*)alloc((size_t)ra * npair * 8);
+            h2d(dA, t->a, (size_t)ra * npair * 8, st);
+            int* d_rowexp = (int*)alloc((size_t)ra * k * 4);
+            d_norm2 = (float*)alloc((size_t)ra * k * 4);
+            packed_rowexp(dA, npair, k, ra, d_rowexp, d_norm2, st);
+            split_packed(SA, dA, npair, k, ra, d_rowexp, ns, st);
+            if (t->rowexp) d2h(t->rowexp, d_rowexp, (size_t)ra * k * 4, st);
+            if (t->rownorm2) d2h(t->rownorm2, d_norm2, (size_t)ra * k * 4, st);
+        } else {
+            double* dA = (double*)alloc((size_t)ra * k * 8);
+            h2d(dA, t->a, (size_t)ra * k * 8, st);
+            if (t->a_rowmax) {     // maxima as a producer would leave them: bit patterns of non-negative doubles
+                split_rows_prepare(SA, ra, k, ns, st);
+                h2d(SA.maxbits, t->a_rowmax, (size_t)ra * 8, st);
+                split_rows_premax(SA, dA, k, ra, k, ns, st);
+            } else {
+                split_rows(SA, dA, k, ra, k, ns, st);
+            }
+        }
+        if (t->qa) d2h(t->qa, SA.q, (size_t)ns * SA.Rp * SA.Kp, st);
+        if (t->ea) d2h(t->ea, SA.E, (size_t)SA.Rp * 4, st);
+        double* dB = nullptr;
+        if (t->stage > 0) {
+            dB = (double*)alloc((size_t)rb * k * 8);
+            h2d(dB, t->b, (size_t)rb * k * 8, st);
+            split_rows(SB, dB, k, rb, k, ns, st);
+            if (t->qb) d2h(t->qb, SB.q, (size_t)ns * SB.Rp * SB.Kp, st);
+            if (t->eb) d2h(t->eb, SB.E, (size_t)SB.Rp * 4, st);
+        }
+        const int rows = t->stage == 1 ? (t->inner > 0 ? t->inner : t->m) : ra;
+        if (t->stage == 1 && t->y_ncolp > 0) {
+            if (!t->packed || t->inner != k || t->a_row0 % k || t->m % k || t->m < k)
+                throw std::runtime_error("fused Y slices need a packed A and whole blocks of tensor rows");
+            double* d_cmax2 = (double*)alloc(8);
+            colnorm_max(dB, k, rb, k, d_cmax2, st);
+            y_prepare(SY, k, t->m / k, t->y_ncolp, ns, d_norm2 + t->a_row0, d_cmax2, st);
+            gemm_ar(SA, t->a_row0, t->m, SB, nullptr, 0, t->inner, st, nullptr, &SY, t->y_ncolp);
+            if (t->qy) d2h(t->qy, SY.q, (size_t)ns * SY.Rp * SY.Kp, st);
+            if (t->ey) d2h(t->ey, SY.E, (size_t)SY.Rp * 4, st);
+        } else if (t->stage > 0) {
+            if (t->stage == 1 && (t->m < 1 || t->inner < 0)) throw std::runtime_error("bad row block");
+            const long ldc = (t->stage == 1 && t->inner > 0) ? (long)((t->m + t->inner - 1) / t->inner) * rb : rb;
+            double* dC = (double*)alloc((size_t)rows * ldc * 8);
+            dev_zero(dC, (size_t)rows * ldc * 8, st);
+            unsigned long long* d_rm = nullptr;
+            if (t->stage == 1 && t->rowmax) { d_rm = (unsigned long long*)alloc((size_t)rows * 8); dev_zero(d_rm, (size_t)rows * 8, st); }
+            if (t->stage == 1) gemm_ar(SA, t->a_row0, t->m, SB, dC, ldc, t->inner, st, d_rm);
+            else gemm_ar_acc(SA, SB, dC, rb, t->symmetric != 0, st, t->kb_per);
+            if (t->c) d2h(t->c, dC, (size_t)rows * ldc * 8, st);
+            if (d_rm) d2h(t->rowmax, d_rm, (size_t)rows * 8, st);
+        }
+        CK(cudaStreamSynchronize(st));
+    } catch (std::exception& e) { set_err(h, e.what()); rc = 2; }
+    SA.release(); SB.release(); SY.release();
+    for (void* p : tmp) dev_free(p);
+    return rc;
+#else
+    set_err(h, "the tensor-core GEMM is not emulated on the CPU");
+    return 3;
+#endif
+}
+
 // C = A B^T through the int8-slice tensor-core path; A [M,K], B [N,K], C [M,N] host fp64 (self-test / tests).
 // symmetric: only the upper triangle of C (M == N) is computed, the rest stays zero.
 extern "C" int b200jk_i8gemm_test(b200jk_handle h, int M, int N, int K, const double* A, const double* B, double* C, int ns,
                                   int symmetric)
 {
-    if (!h) return 1;
-#ifndef B200JK_EMULATE
-    try {
-        using namespace b200jk::i8g;
-        if (ns < 1 || ns > MAXS) throw std::runtime_error("ns out of range");
-        CK(cudaSetDevice(h->device));
-        cudaStream_t st = h->stream;
-        double* dA = (double*)dev_alloc((size_t)M * K * 8);
-        double* dB = (double*)dev_alloc((size_t)N * K * 8);
-        double* dC = (double*)dev_alloc((size_t)M * N * 8);
-        h2d(dA, A, (size_t)M * K * 8, st);
-        h2d(dB, B, (size_t)N * K * 8, st);
-        dev_zero(dC, (size_t)M * N * 8, st);
-        SliceStack SA, SB;
-        split_rows(SA, dA, K, M, K, ns, st);
-        split_rows(SB, dB, K, N, K, ns, st);
-        CK(cudaEventRecord(h->ev0, st));
-        gemm_ar_acc(SA, SB, dC, N, symmetric != 0, st);
-        CK(cudaEventRecord(h->ev1, st));
-        d2h(C, dC, (size_t)M * N * 8, st);
-        CK(cudaStreamSynchronize(st));
-        float ms = 0;
-        CK(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
-        h->stats.ms_kernels = ms;
-        SA.release(); SB.release();
-        dev_free(dA); dev_free(dB); dev_free(dC);
-    } catch (std::exception& e) { set_err(h, e.what()); return 2; }
-    return 0;
-#else
-    (void)M; (void)N; (void)K; (void)A; (void)B; (void)C; (void)ns; (void)symmetric;
-    set_err(h, "the tensor-core GEMM is not emulated on the CPU");
-    return 3;
-#endif
+    b200jk_i8test t{};
+    t.stage = 2; t.ns = ns; t.a = A; t.ra = M; t.k = K; t.b = B; t.rb = N; t.symmetric = symmetric; t.c = C;
+    return b200jk_i8engine_test(h, &t);
 }

@@ -87,7 +87,18 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity)
             : "memory");
     } while (!ok);
 }
+// 2^e for -1022 <= e <= 1023 only (outside, the bit pattern wraps into a wrong value of either sign)
 __device__ __forceinline__ double pow2i(int e) { return __longlong_as_double((long long)(e + 1023) << 52); }
+// x 2^e with one rounding for every int e: one multiply in the range of pow2i, ldexp beyond it, so that a product of two tiny
+// (or huge) row exponents underflows to a subnormal / 0 (overflows to inf) instead of taking the wrapped value of pow2i
+__device__ __forceinline__ double scale2(double x, int e) { return (e >= -1022 && e <= 1023) ? x * pow2i(e) : ldexp(x, e); }
+// the two factors s1 s2 = 2^e, e <= 2046, of a scaling UP that may leave the range of pow2i: x s1 is exact (s1 = 1 unless
+// e > 1023, and then |x| < 2^-975 is lifted into the normal range), so fma(x * s1, s2, c) rounds once, like fma(x, 2^e, c)
+__device__ __forceinline__ void pow2_split(int e, double& s1, double& s2)
+{
+    const int e1 = e > 1023 ? e - 1023 : 0;
+    s1 = pow2i(e1); s2 = pow2i(e - e1);
+}
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int c0, int c1)
@@ -348,8 +359,8 @@ i8gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__
                 for (int j = 0; j < BN / 8; j++) {
                     const int n = nb + 8 * j + cq;
                     if (n >= P.y_ncolp) continue;    // y_ncolp is a multiple of 16: both columns of the pair are inside
-                    double r0 = accv[4 * j + 2 * i] * pow2i(esc + __ldg(P.Eb + n));
-                    double r1 = accv[4 * j + 2 * i + 1] * pow2i(esc + __ldg(P.Eb + n + 1));
+                    double r0 = scale2(accv[4 * j + 2 * i], esc + __ldg(P.Eb + n));
+                    double r1 = scale2(accv[4 * j + 2 * i + 1], esc + __ldg(P.Eb + n + 1));
                     for (int s_ = 0; s_ < NS; s_++) {
                         const double t0 = r0 + 6755399441055744.0, t1 = r1 + 6755399441055744.0;
                         const double q0 = t0 - 6755399441055744.0, q1 = t1 - 6755399441055744.0;
@@ -368,7 +379,7 @@ i8gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__
 #pragma unroll
                     for (int c = 0; c < 2; c++) {
                         const int n = nb + 8 * j + cq + c;
-                        if (n < P.N && (!P.symmetric || n >= m)) atomicAdd(dst + n, accv[4 * j + 2 * i + c] * pow2i(ea + __ldg(P.Eb + n)));
+                        if (n < P.N && (!P.symmetric || n >= m)) atomicAdd(dst + n, scale2(accv[4 * j + 2 * i + c], ea + __ldg(P.Eb + n)));
                     }
                 continue;
             }
@@ -378,15 +389,15 @@ i8gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__
                 const int n = nb + 8 * j + cq;
                 if (n + 1 < P.N && ((off + n) & 1) == 0) {
                     // both columns inside and 16-byte aligned: one 128-bit store
-                    const double v0 = accv[4 * j + 2 * i] * pow2i(ea + __ldg(P.Eb + n));
-                    const double v1 = accv[4 * j + 2 * i + 1] * pow2i(ea + __ldg(P.Eb + n + 1));
+                    const double v0 = scale2(accv[4 * j + 2 * i], ea + __ldg(P.Eb + n));
+                    const double v1 = scale2(accv[4 * j + 2 * i + 1], ea + __ldg(P.Eb + n + 1));
                     *reinterpret_cast<double2*>(dst + n) = make_double2(v0, v1);
                     vmax = fmax(vmax, fmax(fabs(v0), fabs(v1)));
                 } else {
 #pragma unroll
                     for (int c = 0; c < 2; c++)
                         if (n + c < P.N) {
-                            const double v = accv[4 * j + 2 * i + c] * pow2i(ea + __ldg(P.Eb + n + c));
+                            const double v = scale2(accv[4 * j + 2 * i + c], ea + __ldg(P.Eb + n + c));
                             dst[n + c] = v;
                             vmax = fmax(vmax, fabs(v));
                         }
@@ -415,9 +426,8 @@ __global__ void __launch_bounds__(256) split_rows_kernel(const double* __restric
     int e = 0;
     if (mx > 0.0) { frexp(mx, &e); }         // mx = f * 2^e, f in [0.5,1)  =>  |x| / 2^e < 1
     if (lane == 0) E[out_row0 + r] = e;
-    const double sc = ldexp(1.0, 6 - e);
     for (int k = lane; k < Kp; k += 32) {
-        double rr = (k < K) ? x[k] * sc : 0.0;
+        double rr = (k < K) ? scale2(x[k], 6 - e) : 0.0;     // 2^(6-e) alone overflows for a subnormal row maximum
         for (int s = 0; s < ns; s++) {
             double qv = rint(rr);
             out[((long)s * Rp + out_row0 + r) * Kp + k] = (int8_t)(int)qv;
@@ -448,13 +458,12 @@ __global__ void __launch_bounds__(256) split_long_kernel(const double* __restric
     int e = 0;
     if (mx > 0.0) { frexp(mx, &e); }
     if (blockIdx.x == 0 && threadIdx.x == 0) E[r] = e;
-    const double sc = ldexp(1.0, 6 - e);
     // 8 consecutive elements per thread: one 64-bit store per slice (a warp writes 256 contiguous bytes per instruction);
     // k0, k1 and Kp are multiples of 8 (segments of 8192, Kp multiple of 128)
     for (long k = k0 + threadIdx.x * 8L; k < k1; k += 256 * 8L) {
         double rr[8];
 #pragma unroll
-        for (int j = 0; j < 8; j++) rr[j] = (k + j < K) ? x[k + j] * sc : 0.0;
+        for (int j = 0; j < 8; j++) rr[j] = (k + j < K) ? scale2(x[k + j], 6 - e) : 0.0;
         for (int s = 0; s < ns; s++) {
             unsigned long long pack = 0;
 #pragma unroll
@@ -593,11 +602,12 @@ __global__ void __launch_bounds__(256) split_packed_kernel(const double* __restr
             if constexpr (NS7) {
                 // N = rint(x 2^(48-e)), |N| <= 2^48, as (hi, lo) words of the mantissa of x*scale + 1.5*2^52 (offset 2^51 removed):
                 // digit s sits at bit 7(6-s): s = 3..6 in lo[0,28), s = 2 across the words, s = 1 at hi[3,10), s = 0 = hi >> 10 (signed)
-                const double scN = pow2i(48 - e);
+                double s1, scN;
+                pow2_split(48 - e, s1, scN);
                 unsigned lo[4]; int hi[4];
 #pragma unroll
                 for (int j = 0; j < 4; j++) {
-                    const double t_ = fma(pass ? S[c4 + j][rl] : S[rl][c4 + j], scN, 6755399441055744.0);
+                    const double t_ = fma((pass ? S[c4 + j][rl] : S[rl][c4 + j]) * s1, scN, 6755399441055744.0);
                     lo[j] = (unsigned)__double2loint(t_);
                     hi[j] = (__double2hiint(t_) & 0x000FFFFF) - 0x00080000;     // remove exponent bits and the 2^51 offset
                 }
@@ -624,11 +634,12 @@ __global__ void __launch_bounds__(256) split_packed_kernel(const double* __restr
                 // mantissa of x*scale + 1.5*2^52; its digits come out with integer shifts: the top one signed (-64..64), the others
                 // 0..127 (two's-complement style, no carries).  Still an exact representation; the digit products of stage 1 are
                 // bounded by 127*64 instead of 64*64, which the int32 accumulation bound covers up to K = nao < 37 000.
-                const double scN = pow2i(6 - e + 7 * (ns - 1));
+                double s1, scN;
+                pow2_split(6 - e + 7 * (ns - 1), s1, scN);
                 long long N[4];
 #pragma unroll
                 for (int j = 0; j < 4; j++) {
-                    const double t_ = fma(pass ? S[c4 + j][rl] : S[rl][c4 + j], scN, 6755399441055744.0);
+                    const double t_ = fma((pass ? S[c4 + j][rl] : S[rl][c4 + j]) * s1, scN, 6755399441055744.0);
                     N[j] = (long long)(__double_as_longlong(t_) & 0x000FFFFFFFFFFFFFLL) - (1LL << 51);
                 }
                 for (int s_ = 0; s_ < ns; s_++) {
@@ -642,10 +653,11 @@ __global__ void __launch_bounds__(256) split_packed_kernel(const double* __restr
                     *reinterpret_cast<unsigned*>(dst + (long)s_ * Rp * Kp) = pack;
                 }
             } else {
-                const double sc = pow2i(6 - e);
+                double s1, sc;
+                pow2_split(6 - e, s1, sc);
                 double rr[4];
 #pragma unroll
-                for (int j = 0; j < 4; j++) rr[j] = (pass ? S[c4 + j][rl] : S[rl][c4 + j]) * sc;
+                for (int j = 0; j < 4; j++) rr[j] = (pass ? S[c4 + j][rl] : S[rl][c4 + j]) * s1 * sc;
                 for (int s_ = 0; s_ < ns; s_++) {
                     unsigned pack = 0;
 #pragma unroll

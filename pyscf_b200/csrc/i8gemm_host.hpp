@@ -10,6 +10,7 @@ struct SliceStack {      // [ns][Rp][Kp] int8 slices + per-row exponents, device
     size_t cap = 0; int ecap = 0;
     unsigned long long* maxbits = nullptr; size_t maxbits_cap = 0;
     long zeroed_for = 0;      // shape key for which the pads were last zeroed (y_prepare)
+    int dmax = 64;            // largest |digit|: 64 for balanced digits, 127 for the mantissa digits of split_packed (ns <= 7)
     void alloc(int rows, int k, int ns);
     void release();
 };
@@ -27,7 +28,8 @@ void gemm_ar(const SliceStack& A, int a_row0, int M, const SliceStack& B, double
              unsigned long long* rowmax = nullptr, const SliceStack* Yout = nullptr, int y_ncolp = 0);
 void split_rows_prepare(SliceStack& S, int rows, int k, int ns, cudaStream_t st);
 void split_rows_premax(SliceStack& S, const double* X, long ldx, int rows, int k, int ns, cudaStream_t st);
-// C[m*ldc + n] += A B^T (stage 2 of DF-K); upper triangle only when symmetric
-void gemm_ar_acc(const SliceStack& A, const SliceStack& B, double* C, long ldc, bool symmetric, cudaStream_t st);
+// C[m*ldc + n] += A B^T (stage 2 of DF-K); upper triangle only when symmetric.  kb_per > 0 forces K ranges of kb_per K blocks
+// (tests); 0 chooses them to fill whole waves, never longer than the int32 bound allows
+void gemm_ar_acc(const SliceStack& A, const SliceStack& B, double* C, long ldc, bool symmetric, cudaStream_t st, int kb_per = 0);
 }  // namespace i8g
 }  // namespace b200jk

@@ -24,12 +24,24 @@ class Stats(ctypes.Structure):
                 ('n_pairs', ctypes.c_int32)]
 
 
+class I8Test(ctypes.Structure):
+    """b200jk_i8test: arguments and outputs of b200jk_i8engine_test (include/b200jk.h)."""
+    _fields_ = [('stage', ctypes.c_int), ('packed', ctypes.c_int), ('ns', ctypes.c_int),
+                ('a', c_double_p), ('ra', ctypes.c_int), ('k', ctypes.c_int), ('a_rowmax', c_double_p),
+                ('b', c_double_p), ('rb', ctypes.c_int),
+                ('a_row0', ctypes.c_int), ('m', ctypes.c_int), ('inner', ctypes.c_int), ('y_ncolp', ctypes.c_int),
+                ('symmetric', ctypes.c_int), ('kb_per', ctypes.c_int),
+                ('qa', ctypes.c_void_p), ('ea', c_int_p), ('qb', ctypes.c_void_p), ('eb', c_int_p), ('rowexp', c_int_p),
+                ('rownorm2', ctypes.POINTER(ctypes.c_float)),
+                ('c', c_double_p), ('rowmax', c_double_p), ('qy', ctypes.c_void_p), ('ey', c_int_p)]
+
+
 _libs = {}
 
 SYMBOLS = ['b200jk_create', 'b200jk_create2', 'b200jk_destroy', 'b200jk_set_screening', 'b200jk_direct_jk', 'b200jk_direct_jk_device',
            'b200jk_df_build', 'b200jk_df_jk', 'b200jk_df_naux', 'b200jk_get_q_cond', 'b200jk_get_stats',
            'b200jk_last_error', 'b200jk_version', 'b200jk_set_stream', 'b200jk_fp64_peak',
-           'b200jk_set_profile', 'b200jk_get_class_times', 'b200jk_df_get_cderi', 'b200jk_i8gemm_test', 'b200jk_df_set_kmode', 'b200jk_set_shard', 'b200jk_df_jk_device', 'b200jk_df_local_rows',
+           'b200jk_set_profile', 'b200jk_get_class_times', 'b200jk_df_get_cderi', 'b200jk_i8gemm_test', 'b200jk_i8engine_test', 'b200jk_df_set_kmode', 'b200jk_df_set_kblock', 'b200jk_set_shard', 'b200jk_df_jk_device', 'b200jk_df_local_rows',
            'b200jk_df_prepare_j', 'b200jk_df_direct_j', 'b200jk_df_stage_times', 'b200jk_df_set_cderi', 'b200jk_df_get_cderi_cols',
            'b200jk_incore_set_eri', 'b200jk_incore_jk', 'b200jk_set_class_costs']
 
@@ -68,6 +80,8 @@ def load(path=None):
     lib.b200jk_df_get_cderi_cols.argtypes = [vp, c_double_p, ctypes.POINTER(ctypes.c_int64), ctypes.c_int]
     lib.b200jk_i8gemm_test.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_double_p, c_double_p, c_double_p,
                                        ctypes.c_int, ctypes.c_int]
+    lib.b200jk_i8engine_test.argtypes = [vp, ctypes.POINTER(I8Test)]
+    lib.b200jk_df_set_kblock.argtypes = [vp, ctypes.c_int, ctypes.c_int]
     lib.b200jk_df_set_kmode.argtypes = [vp, ctypes.c_int, ctypes.c_int]
     lib.b200jk_df_local_rows.argtypes = [vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]
     lib.b200jk_set_shard.argtypes = [vp, ctypes.c_int, ctypes.c_int]
