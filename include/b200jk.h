@@ -152,6 +152,18 @@ int b200jk_get_class_times(b200jk_handle h, double* ms, int n);
  * max_resident_rows packed rows whose slices stay resident between calls (the rest are re-cut per block); -1 keeps the
  * automatic choice, which a cap can only shrink. */
 int b200jk_df_set_kblock(b200jk_handle h, int max_block_rows, int max_resident_rows);
+/* Tensors larger than the device.  A handle's local rows [0, nrow) are split into device rows [0, n_dev) in HBM and host rows
+ * [n_dev, nrow) in pinned host memory; every J/K call streams the host rows once through two device staging buffers (copies on a
+ * copy stream of the handle, overlapped with the contraction of the previous block) and contracts J and K on each staged block.
+ * The automatic split keeps every row on the device when the tensor fits next to the K workspaces; otherwise it keeps as many as
+ * leave room for them and the staging buffers.  The host part is checked against MemAvailable (/proc/meminfo) first.
+ * set_device_rows: cap on n_dev (-1: automatic), applied by the next b200jk_df_build / b200jk_df_set_cderi (tests, benchmarks).
+ * row_split: n_dev and n_host = nrow - n_dev of the current tensor.
+ * stream_stats: of the last b200jk_df_jk[_device] call: bytes copied host -> device, summed copy time and the part of it the
+ * compute stream waited for (exposed_ms: copy time not hidden behind compute). */
+int b200jk_df_set_device_rows(b200jk_handle h, int max_rows);
+int b200jk_df_row_split(b200jk_handle h, int* n_dev, int* n_host);
+int b200jk_df_stream_stats(b200jk_handle h, int64_t* bytes, double* copy_ms, double* exposed_ms);
 /* Self-test of the int8-slice tensor-core GEMM used by DF-K: C[M,N] = A[M,K] B[N,K]^T with `ns` 7-bit slices (split_rows +
  * gemm_ar_acc with automatic K ranges; upper triangle only when symmetric).  b200jk_i8engine_test with stage 2. */
 int b200jk_i8gemm_test(b200jk_handle h, int M, int N, int K, const double* A, const double* B, double* C, int ns,

@@ -8,6 +8,8 @@
 #include "host_common.hpp"
 #include "df_classes.cuh"
 
+#include <functional>
+
 #ifndef B200JK_EMULATE
 #include <cublas_v2.h>
 #include <cusolverDn.h>
@@ -51,6 +53,13 @@ struct DFState {
     std::vector<int64_t> ao_off_h[NPC];
     int build_rank = 0, build_world = 1, row0 = 0, nrow = 0;   // rows [row0, row0+nrow) of the tensor live on this rank
     double* d_cderi = nullptr;
+    // local rows [0, n_dev) live in d_cderi, rows [n_dev, nrow) in pinned host memory h_cderi; the host rows are streamed
+    // through the two device staging buffers d_stage (stage_rows rows each) once per J/K call.  n_dev == nrow when the
+    // tensor fits next to the K workspaces.
+    int n_dev = 0, stage_rows = 0;
+    double* h_cderi = nullptr;
+    double* d_stage[2] = {nullptr, nullptr};
+    int64_t stream_bytes = 0; double stream_copy_ms = 0.0, stream_exposed_ms = 0.0;   // last J/K call (b200jk_df_stream_stats)
     double omega = 0.0;
     // metric factor kept for the integral-direct J (df_jk.get_j): Cholesky L (GPU: column-major lower, emulation: row-major
     // lower) or, when the metric is not positive definite, W = diag(w)^-1/2 V^T [naux, naux_sph] row-major
@@ -78,6 +87,11 @@ struct DFState {
     i8g::SliceStack SAt;
     // per-stage device timers of the last b200jk_df_jk call (CUDA events on the launching stream, read after the final sync)
     std::vector<cudaEvent_t> tm_ev; std::vector<int> tm_tag; size_t tm_used = 0;
+    // streamed host rows: H2D copies run on cp_stream; per staged block, events at copy start / end and around the wait of
+    // the compute stream (exposed copy time); ev_free[slot] marks the compute on a staging buffer done
+    cudaStream_t cp_stream = nullptr;
+    std::vector<cudaEvent_t> sx_ev;
+    cudaEvent_t ev_free[2] = {nullptr, nullptr};
 #endif
     double stage_ms[B200JK_DF_NSTAGE] = {0}; int stage_n[B200JK_DF_NSTAGE] = {0};
 };
@@ -89,7 +103,14 @@ void df_free(DFState* d)
     if (!d) return;
 #ifndef B200JK_EMULATE
     for (cudaEvent_t e : d->tm_ev) cudaEventDestroy(e);
+    for (cudaEvent_t e : d->sx_ev) cudaEventDestroy(e);
+    for (cudaEvent_t e : d->ev_free) if (e) cudaEventDestroy(e);
+    if (d->cp_stream) cudaStreamDestroy(d->cp_stream);
+    if (d->h_cderi) cudaFreeHost(d->h_cderi);
+#else
+    free(d->h_cderi);
 #endif
+    dev_free(d->d_stage[0]); dev_free(d->d_stage[1]);
     dev_free(d->d_aprims);
     for (int l = 0; l <= LMAX; l++) { dev_free(d->d_akets[l]); dev_free(d->d_aket_off[l]); }
     dev_free(d->d_acart_sh); dev_free(d->d_acart_comp); dev_free(d->d_asph_sh); dev_free(d->d_asph_m);
@@ -440,6 +461,76 @@ static void for_each_j3c_batch(b200jk_handle h, DFState* d, double omega, stream
     dev_free(d_xc); dev_free(d_xa);
 }
 
+// ---- device / host row split ---------------------------------------------------------------------
+// bytes of int8 slices per packed row, and what the K build needs besides the tensor: the per-block slice stack and 12 GB of
+// workspaces (the reserve the slice-residency decision of df_jk_impl keeps)
+static size_t slice_row_bytes(int nao, int ns) { return (size_t)ns * nao * (((size_t)nao + 127) / 128 * 128); }
+static size_t k_reserve_bytes(int nao, int kb, int ns) { return (size_t)(kb + 1) * slice_row_bytes(nao, ns) + (12UL << 30); }
+
+// MemAvailable of /proc/meminfo in bytes (0 when it cannot be read)
+static size_t host_mem_available()
+{
+    FILE* f = fopen("/proc/meminfo", "r");
+    if (!f) return 0;
+    char line[256];
+    size_t kb = 0;
+    while (fgets(line, sizeof line, f))
+        if (sscanf(line, "MemAvailable: %zu kB", &kb) == 1) break;
+    fclose(f);
+    return kb * 1024;
+}
+
+// Decide how many of this rank's nloc rows stay in HBM and allocate d_cderi (zero-filled on request), the pinned host rows and the two
+// staging buffers.  With the automatic split (h->df_dev_rows = -1) every row stays on the device when the tensor fits next to
+// the K reserve; otherwise the device keeps as many rows as leave room for that reserve and the staging buffers.  The host
+// part is checked against MemAvailable before it is allocated; when it does not fit either, the state is freed and the call
+// fails.  Returns an empty string on success, else the error.
+static std::string plan_rows(b200jk_handle h, DFState* d, int nloc, bool zero_fill, stream_t st)
+{
+    const int nao = h->nsph;
+    const size_t rowb = (size_t)d->npair * 8;
+    const size_t stage_cap = std::max<size_t>(1, std::min<size_t>(std::max(nloc, 1), (1UL << 30) / rowb));   // rows in 1 GiB
+    long n_dev = nloc;
+    if (h->df_dev_rows >= 0) n_dev = std::min<long>(nloc, h->df_dev_rows);
+#ifndef B200JK_EMULATE
+    else {
+        size_t freeb = 0, totb = 0;
+        CK(cudaMemGetInfo(&freeb, &totb));
+        const long n2 = (long)nao * nao;
+        const int kb = (int)std::max<long>(1, std::min<long>(std::max(nloc, 1), (2048L << 20) / (n2 * 8)));   // df_jk_impl's K block
+        const double reserve = (double)k_reserve_bytes(nao, kb, d->k_slices);
+        if ((double)nloc * rowb + reserve > (double)freeb) {
+            const double avail = (double)freeb - reserve - 2.0 * stage_cap * rowb - (double)(1UL << 30);
+            n_dev = avail > 0 ? std::min<long>(nloc, (long)(avail / rowb)) : 0;
+        }
+    }
+#endif
+    const long n_host = nloc - n_dev;
+    if (n_host > 0) {
+        const size_t hbytes = (size_t)n_host * rowb, avail = host_mem_available();
+        if (avail && (double)hbytes > 0.9 * (double)avail - (double)(2UL << 30)) {
+            char buf[320];
+            snprintf(buf, sizeof buf, "the DF tensor does not fit: %ld of its %d rows (%.1f GB) exceed the device and need pinned host "
+                     "memory, but MemAvailable is %.1f GB", n_host, nloc, hbytes / 1e9, avail / 1e9);
+            return buf;
+        }
+    }
+    d->n_dev = (int)n_dev;
+    d->d_cderi = (double*)dev_alloc((size_t)std::max<long>(n_dev, 1) * rowb);
+    if (zero_fill) dev_zero(d->d_cderi, (size_t)std::max<long>(n_dev, 1) * rowb, st);
+    if (n_host > 0) {
+        d->stage_rows = (int)std::min<long>((long)stage_cap, n_host);
+#ifndef B200JK_EMULATE
+        CK(cudaHostAlloc((void**)&d->h_cderi, (size_t)n_host * rowb, cudaHostAllocDefault));
+#else
+        d->h_cderi = (double*)malloc((size_t)n_host * rowb);
+        if (!d->h_cderi) throw std::runtime_error("host rows of the DF tensor: out of memory");
+#endif
+        for (double*& s : d->d_stage) s = (double*)dev_alloc((size_t)d->stage_rows * rowb);
+    }
+    return "";
+}
+
 static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, const int32_t* aux_bas, int aux_nbas,
                          const double* aux_env, int aux_nenv, double omega, double lindep, bool j_only)
 {
@@ -616,29 +707,61 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
         const long npair = d->npair;
         const int64_t bcols = std::min<int64_t>(std::max<int64_t>(4096, (int64_t)((3ULL << 30) / ((size_t)d->naux_cart * 8))) + 128, d->rowlen);
         double* d_ybatch = (double*)dev_alloc((size_t)std::max(nloc, 1) * (size_t)bcols * 8);
-        d->d_cderi = (double*)dev_alloc((size_t)std::max(nloc, 1) * npair * 8);
-        dev_zero(d->d_cderi, (size_t)std::max(nloc, 1) * npair * 8, st);
-        for_each_j3c_batch(h, d, omega, st, [&](int64_t col0, int64_t cols, const double* d_xa, int cb, int p0, int p1) {
-            if (nloc <= 0) return;
-            if (cols > bcols) throw std::runtime_error("internal: 3-center batch larger than its scratch buffer");
+        const std::string split_err = plan_rows(h, d, nloc, true, st);
+        if (!split_err.empty()) {
+            dev_free(d_T); dev_free(d_ybatch); dev_free(d_j2c_cart);
+            df_free(d); h->df = nullptr;
+            throw std::runtime_error(split_err);
+        }
+        const int n_dev = d->n_dev, n_host = nloc - n_dev;
+        // rows of the tensor from the rows Trows[nr][nas] of the metric transform into out[nr][npair] (zero-filled)
+        auto fill_rows = [&](const double* Trows, int nr, double* out) {
+            for_each_j3c_batch(h, d, omega, st, [&](int64_t col0, int64_t cols, const double* d_xa, int cb, int p0, int p1) {
+                if (nr <= 0) return;
+                if (cols > bcols) throw std::runtime_error("internal: 3-center batch larger than its scratch buffer");
 #ifndef B200JK_EMULATE
-            // row-major Y[nloc, cols] = T[nloc, nas] . Xa[nas, cols]  <=>  col-major Y^T = Xa^T . T^T
-            const double one = 1.0, zero = 0.0;
-            CKB(cublasDgemm(d->cublas, CUBLAS_OP_N, CUBLAS_OP_N, (int)cols, nloc, nas, &one, d_xa, (int)cols, d_T, nas, &zero,
-                            d_ybatch, (int)cols));
+                // row-major Y[nr, cols] = T[nr, nas] . Xa[nas, cols]  <=>  col-major Y^T = Xa^T . T^T
+                const double one = 1.0, zero = 0.0;
+                CKB(cublasDgemm(d->cublas, CUBLAS_OP_N, CUBLAS_OP_N, (int)cols, nr, nas, &one, d_xa, (int)cols, Trows, nas, &zero,
+                                d_ybatch, (int)cols));
 #else
-            for (int i = 0; i < nloc; i++)
-                for (int64_t c = 0; c < cols; c++) {
-                    double acc = 0.0;
-                    for (int k = 0; k < nas; k++) acc += d_T[(size_t)i * nas + k] * d_xa[(size_t)k * cols + c];
-                    d_ybatch[(size_t)i * cols + c] = acc;
-                }
+                for (int i = 0; i < nr; i++)
+                    for (int64_t c = 0; c < cols; c++) {
+                        double acc = 0.0;
+                        for (int k = 0; k < nas; k++) acc += Trows[(size_t)i * nas + k] * d_xa[(size_t)k * cols + c];
+                        d_ybatch[(size_t)i * cols + c] = acc;
+                    }
 #endif
-            const int la = h->pc[cb].la, lb = h->pc[cb].lb;
-            PairC2SBatchFn p2{d_ybatch, d->d_cderi, cols, col0, npair, h->pc[cb].d_all + p0, d->d_ao_off[cb] + p0, p1 - p0, la, lb,
-                              h->d_sh_sph, h->d_c2s_off, h->d_c2s};
-            launch_1d((long)nloc * (p1 - p0) * (2 * la + 1) * (2 * lb + 1), p2, st);
-        });
+                const int la = h->pc[cb].la, lb = h->pc[cb].lb;
+                PairC2SBatchFn p2{d_ybatch, out, cols, col0, npair, h->pc[cb].d_all + p0, d->d_ao_off[cb] + p0, p1 - p0, la, lb,
+                                  h->d_sh_sph, h->d_c2s_off, h->d_c2s};
+                launch_1d((long)nr * (p1 - p0) * (2 * la + 1) * (2 * lb + 1), p2, st);
+            });
+        };
+        if (n_dev > 0 || n_host == 0) fill_rows(d_T, n_dev, d->d_cderi);
+        if (n_host > 0) {
+            // host rows in blocks as large as the device memory left over allows (the K reserve is not in use yet); the 3-center
+            // integrals are recomputed once per block (d_ybatch holds nloc >= hb rows)
+            long hb = d->stage_rows;
+#ifndef B200JK_EMULATE
+            size_t freeb = 0, totb = 0;
+            CK(cudaMemGetInfo(&freeb, &totb));
+            const double scratch = (double)(d->naux_cart + nas) * bcols * 8 + (double)(1UL << 30);   // for_each_j3c_batch + margin
+            if ((double)freeb > scratch + npair * 8.0) hb = std::max(hb, (long)(((double)freeb - scratch) / (npair * 8.0)));
+#endif
+            hb = std::max(1L, std::min<long>(hb, n_host));
+            double* d_blk = (double*)dev_alloc((size_t)hb * npair * 8);
+            for (int a = n_dev; a < nloc; a += (int)hb) {
+                const int nr = (int)std::min<long>(hb, nloc - a);
+                dev_zero(d_blk, (size_t)nr * npair * 8, st);
+                fill_rows(d_T + (size_t)a * nas, nr, d_blk);
+                d2h(d->h_cderi + (size_t)(a - n_dev) * npair, d_blk, (size_t)nr * npair * 8, st);
+            }
+#ifndef B200JK_EMULATE
+            CK(cudaStreamSynchronize(st));
+#endif
+            dev_free(d_blk);
+        }
         dev_free(d_T);
         dev_free(d_ybatch);
 #ifndef B200JK_EMULATE
@@ -851,8 +974,11 @@ extern "C" int b200jk_df_set_cderi(b200jk_handle h, const double* cderi, int nau
         const int bw = h->shard_world, br = h->shard_rank;
         const int r_lo = (int)((long)naux * br / bw), r_hi = (int)((long)naux * (br + 1) / bw);
         d->build_rank = br; d->build_world = bw; d->row0 = r_lo; d->nrow = r_hi - r_lo;
-        d->d_cderi = (double*)dev_alloc((size_t)std::max(d->nrow, 1) * d->npair * 8);
-        if (d->nrow > 0) h2d(d->d_cderi, cderi + (size_t)r_lo * d->npair, (size_t)d->nrow * d->npair * 8, st);
+        const std::string split_err = plan_rows(h, d, d->nrow, false, st);
+        if (!split_err.empty()) { df_free(d); h->df = nullptr; throw std::runtime_error(split_err); }
+        if (d->n_dev > 0) h2d(d->d_cderi, cderi + (size_t)r_lo * d->npair, (size_t)d->n_dev * d->npair * 8, st);
+        if (d->nrow > d->n_dev)
+            memcpy(d->h_cderi, cderi + (size_t)(r_lo + d->n_dev) * d->npair, (size_t)(d->nrow - d->n_dev) * d->npair * 8);
 #ifndef B200JK_EMULATE
         CK(cudaStreamSynchronize(st));
 #endif
@@ -883,14 +1009,18 @@ extern "C" int b200jk_df_get_cderi_cols(b200jk_handle h, double* out, const int6
             if (cols[c] < 0 || cols[c] >= d->npair) throw std::runtime_error("column index out of range");
         if (d->nrow < 1) return 0;
         static_assert(sizeof(long) == sizeof(int64_t), "LP64");
-        long* d_cols = (long*)dev_alloc((size_t)ncols * 8);
-        double* d_out = (double*)dev_alloc((size_t)d->nrow * ncols * 8);
-        h2d(d_cols, cols, (size_t)ncols * 8);
-        GatherColsFn g{d->d_cderi, d_cols, d_out, d->npair, ncols};
-        launch_1d((long)d->nrow * ncols, g, 0);
-        d2h(out, d_out, (size_t)d->nrow * ncols * 8);
-        dev_sync();
-        dev_free(d_cols); dev_free(d_out);
+        if (d->n_dev > 0) {
+            long* d_cols = (long*)dev_alloc((size_t)ncols * 8);
+            double* d_out = (double*)dev_alloc((size_t)d->n_dev * ncols * 8);
+            h2d(d_cols, cols, (size_t)ncols * 8);
+            GatherColsFn g{d->d_cderi, d_cols, d_out, d->npair, ncols};
+            launch_1d((long)d->n_dev * ncols, g, 0);
+            d2h(out, d_out, (size_t)d->n_dev * ncols * 8);
+            dev_sync();
+            dev_free(d_cols); dev_free(d_out);
+        }
+        for (long r = 0; r < d->nrow - d->n_dev; r++)      // rows in pinned host memory
+            for (int c = 0; c < ncols; c++) out[(d->n_dev + r) * ncols + c] = d->h_cderi[r * d->npair + cols[c]];
     } catch (std::exception& e) { set_err(h, e.what()); return 2; }
     return 0;
 }
@@ -902,8 +1032,13 @@ extern "C" int b200jk_df_get_cderi(b200jk_handle h, double* out, int r0, int nr)
     try {
         DFState* d = h->df;
         if (r0 < 0 || nr < 0 || r0 + nr > d->nrow) throw std::runtime_error("row range out of bounds (rows are local to this rank)");
-        d2h(out, d->d_cderi + (size_t)r0 * d->npair, (size_t)nr * d->npair * 8);
-        dev_sync();
+        const int nd = std::max(0, std::min(r0 + nr, d->n_dev) - r0);     // rows in HBM, then rows in pinned host memory
+        if (nd > 0) {
+            d2h(out, d->d_cderi + (size_t)r0 * d->npair, (size_t)nd * d->npair * 8);
+            dev_sync();
+        }
+        if (nr > nd)
+            memcpy(out + (size_t)nd * d->npair, d->h_cderi + (size_t)(r0 + nd - d->n_dev) * d->npair, (size_t)(nr - nd) * d->npair * 8);
     } catch (std::exception& e) { set_err(h, e.what()); return 2; }
     return 0;
 }
@@ -925,6 +1060,9 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
         if (d->build_world == h->shard_world && d->build_rank == h->shard_rank) { r_lo = 0; r_hi = d->nrow; }
         else if (d->build_world == 1) { r_lo = (int)((long)d->nrow * h->shard_rank / h->shard_world); r_hi = (int)((long)d->nrow * (h->shard_rank + 1) / h->shard_world); }
         else throw std::runtime_error("the tensor was built for a different shard; call b200jk_df_build again after b200jk_set_shard");
+        // rows [r_lo, r_dev) are in d_cderi, rows [r_dev, r_hi) in pinned host memory: streamed through the staging buffers
+        const int r_dev = std::max(r_lo, std::min(r_hi, d->n_dev));
+        const bool streamed = r_dev < r_hi;
 #ifndef B200JK_EMULATE
         CK(cudaSetDevice(h->device));
         cudaStream_t st = h->stream;
@@ -965,40 +1103,39 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
 #else
         auto mark = [&](int) {};
 #endif
-        if (vj) {
-            DmTrilFn tf{d->d_dm, d->d_dmtril, nao, npair};
-            launch_1d((long)n_dm * npair, tf, st); launches++;
-            dev_zero(d->d_vjtril, (size_t)n_dm * npair * 8, st);
+        // ---- host rows: staged blocks of hb rows, block b in staging buffer b & 1.  Blocks 0 and 1 are copied while the
+        //      device rows are contracted; block b + 2 is copied once the compute stream is done with block b.
+        const int hb = streamed ? (d->kb_max > 0 ? std::min(d->stage_rows, d->kb_max) : d->stage_rows) : 0;
+        const int nblk = streamed ? (r_hi - r_dev + hb - 1) / hb : 0;
+        d->stream_bytes = 0; d->stream_copy_ms = 0.0; d->stream_exposed_ms = 0.0;
+        auto blk_rows = [&](int b, int& a, int& nr) { a = r_dev + b * hb; nr = std::min(hb, r_hi - a); };
 #ifndef B200JK_EMULATE
-            dev_zero(d->d_rho, (size_t)n_dm * naux * 8, st);
-            const long seglen = 16384;   // 128 KiB of a row per CTA
-            const unsigned nseg = (unsigned)((npair + seglen - 1) / seglen);
-            // two streaming passes over the tensor (rho, then J): 2 launches, both HBM-bound
-            (void)rb;
-            mark(B200JK_DF_STAGE_J_RHO);
-            for (int r0 = r_lo; r0 < r_hi; r0 += 32768 * DFJ_R) {
-                int nr = std::min(32768 * DFJ_R, r_hi - r0);
-                dfj_rho_kernel<<<dim3(nseg, (nr + DFJ_R - 1) / DFJ_R, n_dm), 256, 0, st>>>(d->d_cderi, d->d_dmtril, d->d_rho, npair, r0, r0 + nr, naux, seglen, npair);
-                launches++;
+        if (streamed) {
+            if (!d->cp_stream) {
+                CK(cudaStreamCreateWithFlags(&d->cp_stream, cudaStreamNonBlocking));
+                for (cudaEvent_t& e : d->ev_free) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
             }
-            mark(B200JK_DF_STAGE_J_ACC);
-            {
-                const unsigned ncb = (unsigned)((npair + 255) / 256);
-                // >= ~6 waves of 8 CTAs per SM, each row range >= 64 rows
-                unsigned gy = (unsigned)std::max<long>(1, std::min<long>((r_hi - r_lo) / 64, (6L * device_sm_count() * 8 + ncb - 1) / ncb));
-                dfj_acc_kernel<<<dim3(ncb, gy), 256, 0, st>>>(d->d_cderi, d->d_rho, d->d_vjtril, npair, r_lo, r_hi - r_lo, naux, n_dm, npair);
-            }
-            launches++;
-            mark(-1);
-            CK(cudaGetLastError());
+            while (d->sx_ev.size() < 4 * (size_t)nblk) { cudaEvent_t e; CK(cudaEventCreate(&e)); d->sx_ev.push_back(e); }
+            CK(cudaStreamWaitEvent(d->cp_stream, h->ev0, 0));     // the copies start inside the bracket of this call
+        }
+        auto issue_copy = [&](int b) {
+            int a, nr;
+            blk_rows(b, a, nr);
+            if (b >= 2) CK(cudaStreamWaitEvent(d->cp_stream, d->ev_free[b & 1], 0));
+            CK(cudaEventRecord(d->sx_ev[4 * b], d->cp_stream));
+            CK(cudaMemcpyAsync(d->d_stage[b & 1], d->h_cderi + (size_t)(a - d->n_dev) * npair, (size_t)nr * npair * 8,
+                               cudaMemcpyHostToDevice, d->cp_stream));
+            CK(cudaEventRecord(d->sx_ev[4 * b + 1], d->cp_stream));
+        };
 #else
-            for (int s = 0; s < n_dm; s++)
-                for (int r = r_lo; r < r_hi; r++) {
-                    double acc = 0;
-                    for (long t = 0; t < npair; t++) acc += d->d_cderi[(size_t)r * npair + t] * d->d_dmtril[(size_t)s * npair + t];
-                    for (long t = 0; t < npair; t++) d->d_vjtril[(size_t)s * npair + t] += acc * d->d_cderi[(size_t)r * npair + t];
-                }
+        auto issue_copy = [&](int b) {
+            int a, nr;
+            blk_rows(b, a, nr);
+            memcpy(d->d_stage[b & 1], d->h_cderi + (size_t)(a - d->n_dev) * npair, (size_t)nr * npair * 8);
+        };
 #endif
+        for (int b = 0; b < std::min(nblk, 2); b++) issue_copy(b);
+        auto finish_j = [&]() {
             UnpackTrilFn uf{d->d_vjtril, d->d_vj, nao, npair};
             launch_1d((long)n_dm * n2, uf, st); launches++;
             if (!on_device) d2h(vj, d->d_vj, (size_t)n_dm * n2 * 8, st);
@@ -1007,10 +1144,60 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
                 CK(cudaMemcpyAsync(vj, d->d_vj, (size_t)n_dm * n2 * 8, cudaMemcpyDeviceToDevice, st));
 #endif
             }
+        };
+#ifndef B200JK_EMULATE
+        const long seglen = 16384;   // 128 KiB of a row per CTA
+        const unsigned nseg = (unsigned)((npair + seglen - 1) / seglen);
+        // J of the rows [r0, r0 + nr) at src (row r0 first): rho, then J~ += rho . rows
+        auto j_rows = [&](const double* src, int r0, int nr) {
+            mark(B200JK_DF_STAGE_J_RHO);
+            for (int q = 0; q < nr; q += 32768 * DFJ_R) {
+                const int m = std::min(32768 * DFJ_R, nr - q);
+                dfj_rho_kernel<<<dim3(nseg, (m + DFJ_R - 1) / DFJ_R, n_dm), 256, 0, st>>>(src, d->d_dmtril, d->d_rho + r0, npair, q, q + m, naux, seglen, npair);
+                launches++;
+            }
+            mark(B200JK_DF_STAGE_J_ACC);
+            const unsigned ncb = (unsigned)((npair + 255) / 256);
+            unsigned gy = (unsigned)std::max<long>(1, std::min<long>(nr / 64, (6L * device_sm_count() * 8 + ncb - 1) / ncb));
+            dfj_acc_kernel<<<dim3(ncb, gy), 256, 0, st>>>(src, d->d_rho + r0, d->d_vjtril, npair, 0, nr, naux, n_dm, npair);
+            launches++;
+            mark(-1);
+            CK(cudaGetLastError());
+        };
+#else
+        auto j_rows = [&](const double* src, int, int nr) {
+            for (int s = 0; s < n_dm; s++)
+                for (int r = 0; r < nr; r++) {
+                    double acc = 0;
+                    for (long t = 0; t < npair; t++) acc += src[(size_t)r * npair + t] * d->d_dmtril[(size_t)s * npair + t];
+                    for (long t = 0; t < npair; t++) d->d_vjtril[(size_t)s * npair + t] += acc * src[(size_t)r * npair + t];
+                }
+        };
+#endif
+        if (vj) {
+            DmTrilFn tf{d->d_dm, d->d_dmtril, nao, npair};
+            launch_1d((long)n_dm * npair, tf, st); launches++;
+            dev_zero(d->d_vjtril, (size_t)n_dm * npair * 8, st);
+#ifndef B200JK_EMULATE
+            dev_zero(d->d_rho, (size_t)n_dm * naux * 8, st);
+#endif
+            // two streaming passes over the device rows (rho, then J): 2 launches, both HBM-bound
+            (void)rb;
+            if (!streamed || r_dev > r_lo) j_rows(d->d_cderi + (size_t)r_lo * npair, r_lo, r_dev - r_lo);
+            if (!streamed) finish_j();
         }
+        const bool use_occ = (occ != nullptr && nocc > 0);
+        const int ncol = use_occ ? nocc : nao;
+#ifndef B200JK_EMULATE
+        // tensor-core engine (k_mode 1): the occupied-orbital algorithm when the density carries its orbitals
+        // (pyscf/df/df_jk.py:339-357), else the general-density algorithm (df_jk.py:382-408) with the density itself as
+        // the right factor: Y[nu,(P,k)] = sum_mu A_P[nu,mu] D[mu,k], K[i,l] = sum_(P,k) Y[i,(P,k)] A_P[l,k] — the same two
+        // int8-slice GEMM stages, no cuBLAS
+        const bool tc = d->k_mode == 1;
+        const bool k_sym = use_occ || hermi == 1;   // the result is symmetric: compute the upper triangle, mirror at the end
+#endif
+        std::function<void(const double*, int, int)> k_block;   // K of the rows [r0, r0 + nr) at src (row r0 first)
         if (vk) {
-            bool use_occ = (occ != nullptr && nocc > 0);
-            int ncol = use_occ ? nocc : nao;
             if ((size_t)kb > d->ws_rows || (size_t)ncol > d->ws_nocc || (size_t)n_dm > d->ws_occ_ndm) {
                 dev_free(d->d_A); dev_free(d->d_Y); dev_free(d->d_occ);
                 d->d_A = (double*)dev_alloc((size_t)kb * nao * ((nao + 15) & ~15) * 8);   // rows of nao columns padded to 16 (general-density G operand)
@@ -1028,12 +1215,6 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
             }
             dev_zero(d->d_vk, (size_t)n_dm * n2 * 8, st);
 #ifndef B200JK_EMULATE
-            // tensor-core engine (k_mode 1): the occupied-orbital algorithm when the density carries its orbitals
-            // (pyscf/df/df_jk.py:339-357), else the general-density algorithm (df_jk.py:382-408) with the density itself as
-            // the right factor: Y[nu,(P,k)] = sum_mu A_P[nu,mu] D[mu,k], K[i,l] = sum_(P,k) Y[i,(P,k)] A_P[l,k] — the same two
-            // int8-slice GEMM stages, no cuBLAS
-            const bool tc = d->k_mode == 1;
-            const bool k_sym = use_occ || hermi == 1;   // the result is symmetric: compute the upper triangle, mirror at the end
             if (tc) {
                 // stage 2 in one K range: pairs(<=ns) * K * 64*64 <= 2^31 - 1 (gemm_ar_acc splits K further where this does not
                 // hold; gemm_ar rejects a stage 1 whose nao breaks the bound)
@@ -1045,7 +1226,8 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
                     d->d_rowexp = (int*)dev_alloc((size_t)std::max(d->nrow, 1) * nao * 4);
                     d->d_rownorm2 = (float*)dev_alloc((size_t)std::max(d->nrow, 1) * nao * 4);
                     d->d_cmax2 = (double*)dev_alloc(8);
-                    i8g::packed_rowexp(d->d_cderi, npair, nao, d->nrow, d->d_rowexp, d->d_rownorm2, st);
+                    if (d->n_dev == d->nrow || d->n_dev > 0)     // host rows: per staged block, every call
+                        i8g::packed_rowexp(d->d_cderi, npair, nao, d->n_dev, d->d_rowexp, d->d_rownorm2, st);
                 }
             }
 #endif
@@ -1059,7 +1241,7 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
                 const size_t kp = ((size_t)nao + 127) / 128 * 128;
                 const size_t per_row = (size_t)d->k_slices * nao * kp;    // bytes of slices per packed row
                 const size_t reserve = (size_t)(kb + 1) * per_row + (12UL << 30);   // the per-block stack + workspaces allocated later
-                const long nloc = r_hi - r_lo;
+                const long nloc = r_dev - r_lo;                       // only rows in HBM can be resident
                 long np = 0;
                 if (freeb * 0.85 > (double)reserve) np = (long)((freeb * 0.85 - (double)reserve) / (double)per_row);
                 if (np >= nloc) np = nloc;
@@ -1077,14 +1259,13 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
                 d->sa_decided = true; d->sa_ns = d->k_slices; d->sa_lo = r_lo; d->sa_hi = r_hi;
             }
 #endif
-            for (int r0 = r_lo; r0 < r_hi; r0 += kb) {
-                int nr = std::min(kb, r_hi - r0);
+            k_block = [&](const double* src, int r0, int nr) {
 #ifndef B200JK_EMULATE
                 const bool blk_resident = tc && (r0 - r_lo + nr <= d->sa_np);
                 if (tc) {
                     if (!blk_resident) {    // slices of this block straight from the packed rows
                         mark(B200JK_DF_STAGE_K_SLICE);
-                        i8g::split_packed(d->SAt, d->d_cderi + (size_t)r0 * npair, npair, nao, nr, d->d_rowexp + (size_t)r0 * nao, d->k_slices, st);
+                        i8g::split_packed(d->SAt, src, npair, nao, nr, d->d_rowexp + (size_t)r0 * nao, d->k_slices, st);
                         mark(-1);
                         launches++;
                     }
@@ -1093,18 +1274,18 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
                         // same (P, k) column layout as Y: k padded to 16 when stage 1 cuts the slices of Y itself
                         static const bool fuse_y_g = getenv("B200JK_NO_YFUSE") == nullptr;
                         const int gcol = fuse_y_g ? ((nao + 15) & ~15) : nao;
-                        UnpackLongFn ul{d->d_cderi, d->d_A, nao, npair, r0, (long)nr * gcol, gcol};
+                        UnpackLongFn ul{src, d->d_A, nao, npair, 0, (long)nr * gcol, gcol};
                         launch_1d((long)nao * nr * gcol, ul, st);
                         i8g::split_rows(d->SG, d->d_A, (long)nr * gcol, nao, nr * gcol, d->k_slices, st);
                         mark(-1);
                         launches += 2;
                     }
                 } else {
-                    UnpackFn up{d->d_cderi, d->d_A, nao, npair, r0};
+                    UnpackFn up{src, d->d_A, nao, npair, 0};
                     launch_1d((long)nr * n2, up, st); launches++;
                 }
 #else
-                UnpackFn up{d->d_cderi, d->d_A, nao, npair, r0};
+                UnpackFn up{src, d->d_A, nao, npair, 0};
                 launch_1d((long)nr * n2, up, st); launches++;
 #endif
                 for (int s = 0; s < n_dm; s++) {
@@ -1227,7 +1408,35 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
                     }
 #endif
                 }
+            };
+            for (int r0 = r_lo; r0 < r_dev; r0 += kb) k_block(d->d_cderi + (size_t)r0 * npair, r0, std::min(kb, r_dev - r0));
+        }
+        if (streamed) {
+            for (int b = 0; b < nblk; b++) {
+                int r0, nr;
+                blk_rows(b, r0, nr);
+                const double* src = d->d_stage[b & 1];
+#ifndef B200JK_EMULATE
+                CK(cudaEventRecord(d->sx_ev[4 * b + 2], st));
+                CK(cudaStreamWaitEvent(st, d->sx_ev[4 * b + 1], 0));
+                CK(cudaEventRecord(d->sx_ev[4 * b + 3], st));
+#endif
+                if (vj) j_rows(src, r0, nr);
+                if (vk) {
+#ifndef B200JK_EMULATE
+                    if (tc) { i8g::packed_rowexp(src, npair, nao, nr, d->d_rowexp + (size_t)r0 * nao, d->d_rownorm2 + (size_t)r0 * nao, st); launches++; }
+#endif
+                    for (int q = 0; q < nr; q += kb) k_block(src + (size_t)q * npair, r0 + q, std::min(kb, nr - q));
+                }
+#ifndef B200JK_EMULATE
+                CK(cudaEventRecord(d->ev_free[b & 1], st));
+#endif
+                if (b + 2 < nblk) issue_copy(b + 2);
+                d->stream_bytes += (int64_t)nr * npair * 8;
             }
+            if (vj) finish_j();
+        }
+        if (vk) {
 #ifndef B200JK_EMULATE
             if (tc && k_sym) { MirrorUpperFn mf{d->d_vk, nao}; for (int s = 0; s < n_dm; s++) { mf.a = d->d_vk + (size_t)s * n2; launch_1d(n2, mf, st); launches++; } }
 #endif
@@ -1251,6 +1460,12 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
             float t = 0;
             CK(cudaEventElapsedTime(&t, d->tm_ev[i], d->tm_ev[i + 1]));
             d->stage_ms[tag] += t; d->stage_n[tag]++;
+        }
+        for (int b = 0; b < nblk; b++) {
+            float tc_ = 0, tw = 0;
+            CK(cudaEventElapsedTime(&tc_, d->sx_ev[4 * b], d->sx_ev[4 * b + 1]));
+            CK(cudaEventElapsedTime(&tw, d->sx_ev[4 * b + 2], d->sx_ev[4 * b + 3]));
+            d->stream_copy_ms += tc_; d->stream_exposed_ms += tw;
         }
 #endif
         auto t1 = std::chrono::steady_clock::now();
@@ -1290,6 +1505,28 @@ extern "C" int b200jk_df_set_kblock(b200jk_handle h, int max_block_rows, int max
 #ifndef B200JK_EMULATE
     h->df->sa_decided = false;     // the resident stack is re-cut on the next K build
 #endif
+    return 0;
+}
+
+extern "C" int b200jk_df_set_device_rows(b200jk_handle h, int max_rows)
+{
+    if (!h) return 1;
+    if (max_rows < -1) { set_err(h, "bad device row cap"); return 1; }
+    h->df_dev_rows = max_rows;
+    return 0;
+}
+
+extern "C" int b200jk_df_row_split(b200jk_handle h, int* n_dev, int* n_host)
+{
+    if (!h || !h->df || !n_dev || !n_host) { set_err(h, "call b200jk_df_build first"); return 1; }
+    *n_dev = h->df->n_dev; *n_host = h->df->nrow - h->df->n_dev;
+    return 0;
+}
+
+extern "C" int b200jk_df_stream_stats(b200jk_handle h, int64_t* bytes, double* copy_ms, double* exposed_ms)
+{
+    if (!h || !h->df || !bytes || !copy_ms || !exposed_ms) { set_err(h, "call b200jk_df_build first"); return 1; }
+    *bytes = h->df->stream_bytes; *copy_ms = h->df->stream_copy_ms; *exposed_ms = h->df->stream_exposed_ms;
     return 0;
 }
 

@@ -190,6 +190,7 @@ struct b200jk_handle_s {
     int shard_rank = 0, shard_world = 1;   // multi-GPU work partition (b200jk_set_shard)
     DFState* df = nullptr;          // density-fitting state (df.cu)
     void (*df_free)(DFState*) = nullptr;
+    int df_dev_rows = -1;           // b200jk_df_set_device_rows: cap on the tensor rows kept in HBM (-1: automatic)
     double class_ms[NPC * NPC] = {0};
     double class_cost[NPC * NPC] = {0};   // measured class times handed in by the caller (b200jk_set_class_costs); 0 = use the model
     bool have_costs = false;

@@ -7,7 +7,8 @@ Mirrors (names, argument meaning, shapes):
   * addons.make_auxmol / predefined auxiliary basis                    pyscf/df/addons.py:230-361
   * density_fit(mf) installer                                          pyscf/df/df_jk.py:31-107
 The three-index tensor is built on the GPU (Rys kernels + cuSOLVER/cuBLAS for the metric) and stays
-resident in HBM in the reference layout cderi[naux, nao(nao+1)/2].
+resident in HBM in the reference layout cderi[naux, nao(nao+1)/2]; the rows of a tensor larger than the GPU that do not fit
+live in pinned host memory and are streamed through the GPU once per J/K call (set_device_rows, row_split).
 """
 import ctypes
 
@@ -34,6 +35,7 @@ class DF:
         self.blockdim = 240        # pyscf/df/df.py:95 (loop() default block size)
         self.k_engine = 'tcgen05'
         self.k_slices = 7
+        self.device_rows = -1      # cap on the tensor rows kept in HBM, the rest in pinned host memory (-1: automatic)
         self.verbose = getattr(mol, 'verbose', 0)
         self.stdout = getattr(mol, 'stdout', None)
         self.max_memory = getattr(mol, 'max_memory', 4000)
@@ -55,6 +57,7 @@ class DF:
         if self.shard is not None:
             h.check(h.lib.b200jk_set_shard(h._h, int(self.shard[0]), int(self.shard[1])), 'b200jk_set_shard')
         self._built_omega = omega
+        h.check(h.lib.b200jk_df_set_device_rows(h._h, int(self.device_rows)), 'b200jk_df_set_device_rows')
         h.check(h.lib.b200jk_df_build(h._h, _lib.iptr(atm), len(atm), _lib.iptr(bas), len(bas), _lib.dptr(env), len(env),
                                       omega, self.lindep), 'b200jk_df_build')
         self._handle = h
@@ -85,6 +88,7 @@ class DF:
         h = _lib.Handle(mol._atm, mol._bas, np.array(mol._env, dtype=np.float64), device=self.device, libpath=self._libpath)
         if self.shard is not None:
             h.check(h.lib.b200jk_set_shard(h._h, int(self.shard[0]), int(self.shard[1])), 'b200jk_set_shard')
+        h.check(h.lib.b200jk_df_set_device_rows(h._h, int(self.device_rows)), 'b200jk_df_set_device_rows')
         h.check(h.lib.b200jk_df_set_cderi(h._h, _lib.dptr(c), c.shape[0], nao), 'b200jk_df_set_cderi')
         self._handle = h
         self.nao = nao
@@ -105,6 +109,28 @@ class DF:
             h = self._handle
             h.check(h.lib.b200jk_df_set_kmode(h._h, 1 if engine == 'tcgen05' else 0, nslices), 'b200jk_df_set_kmode')
         return self
+
+    def set_device_rows(self, n=-1):
+        """Keep at most `n` rows of this rank's tensor in HBM and the rest in pinned host memory, streamed through the GPU
+        once per J/K call (-1: automatic, every row on the device when the tensor fits).  Applied at the next build."""
+        self.device_rows = -1 if n is None else int(n)
+        return self
+
+    def row_split(self):
+        """(rows in HBM, rows in pinned host memory) of this rank's tensor."""
+        self.get_naoaux()
+        h = self._handle
+        n_dev, n_host = ctypes.c_int(0), ctypes.c_int(0)
+        h.check(h.lib.b200jk_df_row_split(h._h, ctypes.byref(n_dev), ctypes.byref(n_host)), 'b200jk_df_row_split')
+        return n_dev.value, n_host.value
+
+    def stream_stats(self):
+        """Host rows streamed by the last get_jk: {'bytes', 'copy_ms', 'exposed_ms'} (exposed: copy time not hidden
+        behind compute)."""
+        h = self._handle
+        b, c, e = ctypes.c_int64(0), ctypes.c_double(0), ctypes.c_double(0)
+        h.check(h.lib.b200jk_df_stream_stats(h._h, ctypes.byref(b), ctypes.byref(c), ctypes.byref(e)), 'b200jk_df_stream_stats')
+        return {'bytes': b.value, 'copy_ms': c.value, 'exposed_ms': e.value}
 
     def reset(self, mol=None):
         if mol is not None:
@@ -179,6 +205,7 @@ class DF:
             rsh.omega = key
             rsh.lindep = self.lindep
             rsh.k_engine, rsh.k_slices = self.k_engine, self.k_slices
+            rsh.device_rows = self.device_rows
             self._rsh_df[key] = rsh.build()
         return self._rsh_df[key]
 
