@@ -164,6 +164,16 @@ int b200jk_df_set_kblock(b200jk_handle h, int max_block_rows, int max_resident_r
 int b200jk_df_set_device_rows(b200jk_handle h, int max_rows);
 int b200jk_df_row_split(b200jk_handle h, int* n_dev, int* n_host);
 int b200jk_df_stream_stats(b200jk_handle h, int64_t* bytes, double* copy_ms, double* exposed_ms);
+/* Pair screening of the tensor (opt-in; the reference has no such screening).  With tol > 0 the next b200jk_df_build keeps only
+ * the packed AO-pair columns (mu >= nu) whose device shell pair has a Schwarz bound q = sqrt((ab|ab)) >= tol, computed for the
+ * tensor's own operator (omega) in the normalisation of b200jk_set_screening; the handle's 4-center screening state is left as
+ * it is.  Dropped pairs are never integrated; device rows, pinned host rows and staging buffers hold ncol columns per row.
+ * A dropped column has 2-norm <= q < tol, since ||B[:, mu nu]||^2 = (mu nu|P) M^-1 (P|mu nu) <= (mu nu|mu nu).  J of a dropped
+ * pair is 0.  b200jk_df_get_cderi / _cols still return the reference layout, exact zeros at dropped columns.  tol <= 0 (the
+ * default) builds the dense tensor; a tensor handed in by b200jk_df_set_cderi is always dense.
+ * pair_stats: ncol kept columns of the current tensor and npair = nao(nao+1)/2. */
+int b200jk_df_set_pair_tol(b200jk_handle h, double tol);
+int b200jk_df_pair_stats(b200jk_handle h, int64_t* ncol, int64_t* npair);
 /* Self-test of the int8-slice tensor-core GEMM used by DF-K: C[M,N] = A[M,K] B[N,K]^T with `ns` 7-bit slices (split_rows +
  * gemm_ar_acc with automatic K ranges; upper triangle only when symmetric).  b200jk_i8engine_test with stage 2. */
 int b200jk_i8gemm_test(b200jk_handle h, int M, int N, int K, const double* A, const double* B, double* C, int ns,

@@ -51,6 +51,20 @@ struct DFState {
     int64_t* d_pairoff = nullptr;
     long npair = 0;
     std::vector<int64_t> ao_off_h[NPC];
+    // pair screening (b200jk_df_set_pair_tol): a row holds only the ncol packed columns whose device shell pair has a Schwarz
+    // bound q >= pair_tol, in ascending packed order; col_of[npair] (-1: dropped) and pk_of[ncol] map between the two layouts.
+    // Without screening ncol == npair and there are no maps (d_col_of == nullptr).  The build integrates only the kept shell
+    // pairs: kpairs / koff are their per-class lists and Cartesian column offsets (the role of pc[c].d_all / d_ao_off).
+    long ncol = 0;
+    double pair_tol = 0.0;
+    int* d_col_of = nullptr;
+    int64_t* d_pk_of = nullptr;
+    std::vector<int> col_of_h;
+    std::vector<int64_t> pk_of_h;
+    bool pair_screened = false;
+    ShellPair* d_kpairs[NPC] = {nullptr};
+    int64_t* d_koff[NPC] = {nullptr};
+    std::vector<int64_t> koff_h[NPC];
     int build_rank = 0, build_world = 1, row0 = 0, nrow = 0;   // rows [row0, row0+nrow) of the tensor live on this rank
     double* d_cderi = nullptr;
     // local rows [0, n_dev) live in d_cderi, rows [n_dev, nrow) in pinned host memory h_cderi; the host rows are streamed
@@ -115,7 +129,8 @@ void df_free(DFState* d)
     for (int l = 0; l <= LMAX; l++) { dev_free(d->d_akets[l]); dev_free(d->d_aket_off[l]); }
     dev_free(d->d_acart_sh); dev_free(d->d_acart_comp); dev_free(d->d_asph_sh); dev_free(d->d_asph_m);
     dev_free(d->d_ash_l); dev_free(d->d_ash_cart); dev_free(d->d_ash_sph);
-    for (int c = 0; c < NPC; c++) dev_free(d->d_ao_off[c]);
+    for (int c = 0; c < NPC; c++) { dev_free(d->d_ao_off[c]); dev_free(d->d_kpairs[c]); dev_free(d->d_koff[c]); }
+    dev_free(d->d_col_of); dev_free(d->d_pk_of);
     dev_free(d->d_pairoff); dev_free(d->d_cderi); dev_free(d->d_fac); dev_free(d->d_W); dev_free(d->d_Linv);
     dev_free(d->d_dmtril); dev_free(d->d_rho); dev_free(d->d_vjtril); dev_free(d->d_A); dev_free(d->d_Y); dev_free(d->d_occ);
     dev_free(d->d_dm); dev_free(d->d_vk); dev_free(d->d_vj); dev_free(d->d_Y2); dev_free(d->d_occT);
@@ -152,10 +167,12 @@ struct AuxC2SFn {
 // in: [nrow, cols] row-major, the Cartesian (a,b) block of pair p starts at column off[p] - col0, element X[b*nca + a].
 // One thread per (row, pair, m_a, m_b); every (mu >= nu) element of the packed row is produced by exactly one shell pair
 // (elements of shell pairs without surviving primitives are never written: the tensor is zero-filled beforehand).
+// npair is the row length of out; with pair screening (col_of != nullptr) the element goes to column col_of[packed index].
 struct PairC2SBatchFn {
     const double* in; double* out; int64_t cols, col0; long npair;
     const ShellPair* pairs; const int64_t* off; int np; int la, lb;
     const int *sh_sph, *c2s_off; const double* c2s;
+    const int* col_of;
     B2_HD void operator()(long idx) const
     {
         const int nsa = 2 * la + 1, nsb = 2 * lb + 1, nca = (la + 1) * (la + 2) / 2, ncb = (lb + 1) * (lb + 2) / 2;
@@ -178,16 +195,19 @@ struct PairC2SBatchFn {
             for (int a = 0; a < nca; a++) acc += Ta[a] * tb * X[b * nca + a];
         }
         const long hi = mu >= nu ? mu : nu, lo = mu >= nu ? nu : mu;
-        out[r * npair + hi * (hi + 1) / 2 + lo] = acc;
+        const long t = hi * (hi + 1) / 2 + lo;
+        out[r * npair + (col_of ? (long)col_of[t] : t)] = acc;
     }
 };
 
 // dmtril[s][t] = D[mu,nu] + D[nu,mu] (diagonal once)      <- pyscf/df/df_jk.py:329-332
+// npair is the row length of out; with pair screening (pk_of != nullptr) column c holds the packed element pk_of[c]
 struct DmTrilFn {
-    const double* dm; double* out; int nao; long npair;
+    const double* dm; double* out; int nao; long npair; const int64_t* pk_of;
     B2_HD void operator()(long idx) const
     {
         long s = idx / npair, t = idx - s * npair;
+        if (pk_of) t = pk_of[t];
         long mu = (long)((sqrt(8.0 * (double)t + 1.0) - 1.0) * 0.5);
         while ((mu + 1) * (mu + 2) / 2 <= t) mu++;
         while (mu * (mu + 1) / 2 > t) mu--;
@@ -197,28 +217,36 @@ struct DmTrilFn {
     }
 };
 
-// unpack rows [r0, r0+nr) of the packed tensor into full symmetric nao x nao matrices
+// element t (packed index) of a tensor row of length npair: the row itself, or through col_of with 0 for a dropped column
+B2_HD double packed_elem(const double* row, const int* col_of, long t)
+{
+    if (!col_of) return row[t];
+    const int c = col_of[t];
+    return c >= 0 ? row[c] : 0.0;
+}
+
+// unpack rows [r0, r0+nr) of the packed tensor (rows of length npair; col_of: pair-screened rows) into full symmetric nao x nao matrices
 struct UnpackFn {
-    const double* cderi; double* A; int nao; long npair; long r0;
+    const double* cderi; double* A; int nao; long npair; long r0; const int* col_of;
     B2_HD void operator()(long idx) const
     {
         long n2 = (long)nao * nao;
         long r = idx / n2, e = idx - r * n2;
         long i = e / nao, j = e - i * nao;
         long mu = i >= j ? i : j, nu = i >= j ? j : i;
-        A[idx] = cderi[(r0 + r) * npair + mu * (mu + 1) / 2 + nu];
+        A[idx] = packed_elem(cderi + (r0 + r) * npair, col_of, mu * (mu + 1) / 2 + nu);
     }
 };
 
 struct UnpackLongFn {   // G[l][P * ncolp + k] = A_P[l][k] (0 for the pad columns k >= nao) from the packed rows r0 + P: the block as nao long rows
-    const double* tril; double* out; int nao; long npair; int r0; long ld; int ncolp;
+    const double* tril; double* out; int nao; long npair; int r0; long ld; int ncolp; const int* col_of;
     B2_HD void operator()(long idx) const
     {
         long l = idx / ld, e = idx - l * ld;
         long P = e / ncolp, k = e - P * ncolp;
         if (k >= nao) { out[idx] = 0.0; return; }
         long hi = l >= k ? l : k, lo = l >= k ? k : l;
-        out[idx] = tril[(r0 + P) * npair + hi * (hi + 1) / 2 + lo];
+        out[idx] = packed_elem(tril + (r0 + P) * npair, col_of, hi * (hi + 1) / 2 + lo);
     }
 };
 struct IdentityFn { double* a; int n; B2_HD void operator()(long i) const { a[i * (long)n + i] = 1.0; } };
@@ -235,15 +263,15 @@ struct MirrorUpperFn {  // fill the strict lower triangle from the upper one
     B2_HD void operator()(long idx) const { long i = idx / n, j = idx - i * n; if (j < i) a[idx] = a[j * (long)n + i]; }
 };
 
-struct UnpackTrilFn {   // vj[s][i][j] from vjtril[s][t]
-    const double* tril; double* out; int nao; long npair;
+struct UnpackTrilFn {   // vj[s][i][j] from vjtril[s][t] (rows of length npair; col_of: kept columns only, 0 for a dropped pair)
+    const double* tril; double* out; int nao; long npair; const int* col_of;
     B2_HD void operator()(long idx) const
     {
         long n2 = (long)nao * nao;
         long s = idx / n2, e = idx - s * n2;
         long i = e / nao, j = e - i * nao;
         long mu = i >= j ? i : j, nu = i >= j ? j : i;
-        out[idx] = tril[s * npair + mu * (mu + 1) / 2 + nu];
+        out[idx] = packed_elem(tril + s * npair, col_of, mu * (mu + 1) / 2 + nu);
     }
 };
 
@@ -424,16 +452,19 @@ void cpu_cholesky_lower(std::vector<double>& a, int n, bool& ok)
 // ------------------------------------------------------------------------------------------------
 // (ij|P) for all AO shell pairs in batches of bounded scratch: Cartesian rows d_xc[naux_cart, cols] -> spherical aux rows
 // d_xa[naux_sph, cols]; use(col0, cols) consumes one batch (columns = Cartesian pair blocks, DFState::ao_off_h).
+// kept: only the shell pairs that survive pair screening (DFState::kpairs / koff_h), else all of them.
 template <class F>
-static void for_each_j3c_batch(b200jk_handle h, DFState* d, double omega, stream_t st, F use)
+static void for_each_j3c_batch(b200jk_handle h, DFState* d, double omega, stream_t st, F use, bool kept = false)
 {
     const int nac = d->naux_cart, nas = d->naux_sph;
     const int64_t budget_cols = std::max<int64_t>(4096, (int64_t)((3ULL << 30) / ((size_t)nac * 8)));
     double* d_xc = (double*)dev_alloc((size_t)nac * (size_t)std::min<int64_t>(budget_cols + 128, d->rowlen) * 8);
     double* d_xa = (double*)dev_alloc((size_t)nas * (size_t)std::min<int64_t>(budget_cols + 128, d->rowlen) * 8);
     for (int cb = 0; cb < NPC; cb++) {
-        const auto& offs = d->ao_off_h[cb];
-        const int np_all = (int)h->pc[cb].all.size();
+        const auto& offs = kept ? d->koff_h[cb] : d->ao_off_h[cb];
+        const ShellPair* pairs = kept ? d->d_kpairs[cb] : h->pc[cb].d_all;
+        const int64_t* d_off = kept ? d->d_koff[cb] : d->d_ao_off[cb];
+        const int np_all = (int)offs.size();
         if (np_all == 0) continue;
         const int64_t blk = (int64_t)ncart(h->pc[cb].la) * ncart(h->pc[cb].lb);
         int p0 = 0;
@@ -443,7 +474,7 @@ static void for_each_j3c_batch(b200jk_handle h, DFState* d, double omega, stream
             for (int lk = 0; lk <= LMAX; lk++) {
                 if (d->akets[lk].empty()) continue;
                 J3cParams P{};
-                P.bra_pairs = h->pc[cb].d_all + p0; P.nbra = p1 - p0; P.bra_out_off = d->d_ao_off[cb] + p0;
+                P.bra_pairs = pairs + p0; P.nbra = p1 - p0; P.bra_out_off = d_off + p0;
                 P.ket_shells = d->d_akets[lk]; P.nket = (int)d->akets[lk].size();
                 P.bra_prims = h->d_prims; P.ket_prims = d->d_aprims;
                 P.tb = h->tb; P.omega = omega; P.out = d_xc; P.row_stride = cols; P.col0 = col0;
@@ -488,7 +519,7 @@ static size_t host_mem_available()
 static std::string plan_rows(b200jk_handle h, DFState* d, int nloc, bool zero_fill, stream_t st)
 {
     const int nao = h->nsph;
-    const size_t rowb = (size_t)d->npair * 8;
+    const size_t rowb = (size_t)d->ncol * 8;
     const size_t stage_cap = std::max<size_t>(1, std::min<size_t>(std::max(nloc, 1), (1UL << 30) / rowb));   // rows in 1 GiB
     long n_dev = nloc;
     if (h->df_dev_rows >= 0) n_dev = std::min<long>(nloc, h->df_dev_rows);
@@ -531,6 +562,72 @@ static std::string plan_rows(b200jk_handle h, DFState* d, int nloc, bool zero_fi
     return "";
 }
 
+// Pair screening of the tensor's columns: the Schwarz bound q = sqrt((ab|ab)) of every device shell pair for the tensor's own
+// operator (SchwarzSphFn: the reference's normalisation, per segment of a general contraction, as b200jk_set_screening computes
+// it, but on a copy of the pair list so that the 4-center screening state of the handle is left as it is).  A packed column
+// (mu >= nu) is kept iff the q of its shell pair is >= tol; ||B[:, mu nu]||_2^2 = (mu nu|P) M^-1 (P|mu nu) <= (mu nu|mu nu)
+// bounds a dropped column by q < tol.  Shell pairs without a surviving primitive pair are not in pc[c].all: always dropped.
+// Fills ncol, col_of / pk_of (host and device) and the per-class kept pair lists with their Cartesian column offsets.
+static void select_pairs(b200jk_handle h, DFState* d, double omega, double tol, stream_t st)
+{
+    const long npair = d->npair;
+    std::vector<char> keep((size_t)npair, 0);
+    int64_t off = 0;
+    for (int c = 0; c < NPC; c++) {
+        PairClass& P = h->pc[c];
+        std::vector<ShellPair> pairs = P.all;
+        std::vector<int64_t> koff;
+        if (!pairs.empty()) {
+            ShellPair* d_tmp = upload(pairs);
+            const long ne = (long)ncart(P.la) * ncart(P.lb);
+            const long chunk = std::max<long>(1, (256L << 20) / (ne * ne * 8));     // <= 256 MB of scratch per launch
+            double* scratch = (double*)dev_alloc((size_t)std::min<long>(chunk, (long)pairs.size()) * ne * ne * 8);
+            for (long i0 = 0; i0 < (long)pairs.size(); i0 += chunk) {
+                const long n = std::min<long>(chunk, (long)pairs.size() - i0);
+                SchwarzSphFn fn{d_tmp + i0, h->d_prims, h->tb, omega, P.la, P.lb, h->d_c2s + h->c2s_off[P.la], h->d_c2s + h->c2s_off[P.lb],
+                                scratch, 2 * P.la + 1, 2 * P.lb + 1};
+                launch_1d(n, fn, st);
+#ifndef B200JK_EMULATE
+                CK(cudaStreamSynchronize(st));
+#endif
+            }
+            d2h(pairs.data(), d_tmp, pairs.size() * sizeof(ShellPair), st);
+#ifndef B200JK_EMULATE
+            CK(cudaStreamSynchronize(st));
+#endif
+            dev_free(scratch); dev_free(d_tmp);
+        }
+        std::vector<ShellPair> kept;
+        for (const ShellPair& sp : pairs) {
+            if (!(sp.q >= tol)) continue;
+            kept.push_back(sp);
+            koff.push_back(off);
+            off += ncart(P.la) * ncart(P.lb);
+            const DevShell &a = h->sh[sp.ish], &b = h->sh[sp.jsh];
+            for (int ma = 0; ma < 2 * a.l + 1; ma++)
+                for (int mb = 0; mb < 2 * b.l + 1; mb++) {
+                    const long mu = a.sph_off + ma, nu = b.sph_off + mb;
+                    if (sp.ish == sp.jsh && mu < nu) continue;
+                    const long hi = std::max(mu, nu), lo = std::min(mu, nu);
+                    keep[(size_t)(hi * (hi + 1) / 2 + lo)] = 1;
+                }
+        }
+        d->d_kpairs[c] = upload(kept);
+        d->d_koff[c] = upload(koff);
+        d->koff_h[c] = koff;
+    }
+    d->col_of_h.assign((size_t)npair, -1);
+    d->pk_of_h.clear();
+    for (long t = 0; t < npair; t++)
+        if (keep[(size_t)t]) { d->col_of_h[(size_t)t] = (int)d->pk_of_h.size(); d->pk_of_h.push_back(t); }
+    d->ncol = (long)d->pk_of_h.size();
+    if (d->ncol == 0) throw std::runtime_error("pair screening: no AO-pair column has a Schwarz bound >= pair_tol");
+    d->d_col_of = upload(d->col_of_h);
+    d->d_pk_of = upload(d->pk_of_h);
+    d->pair_screened = true;
+    d->pair_tol = tol;
+}
+
 static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, const int32_t* aux_bas, int aux_nbas,
                          const double* aux_env, int aux_nenv, double omega, double lindep, bool j_only)
 {
@@ -569,6 +666,8 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
         }
         d->rowlen = off;
         d->d_pairoff = upload(pairoff);
+        d->ncol = d->npair;
+        if (!j_only && h->df_pair_tol > 0.0) select_pairs(h, d, omega, h->df_pair_tol, st);
 
         // ---- (P|Q) in the Cartesian aux basis, then to spherical
         const int nac = d->naux_cart, nas = d->naux_sph;
@@ -704,7 +803,7 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
         // ---- (ij|P) in batches of AO shell pairs (bounded scratch): Cartesian rows -> spherical aux -> T . (P|ij) -> packed
         //      spherical columns of this batch.  Nothing of size naux x (all Cartesian pairs) ever exists: the largest buffers are
         //      the tensor itself and three batch-sized scratch arrays (<= ~3 GB each), so a 111 GB tensor fits one 180 GB GPU.
-        const long npair = d->npair;
+        const long ncol = d->ncol;   // row length: every packed column, or the kept ones under pair screening
         const int64_t bcols = std::min<int64_t>(std::max<int64_t>(4096, (int64_t)((3ULL << 30) / ((size_t)d->naux_cart * 8))) + 128, d->rowlen);
         double* d_ybatch = (double*)dev_alloc((size_t)std::max(nloc, 1) * (size_t)bcols * 8);
         const std::string split_err = plan_rows(h, d, nloc, true, st);
@@ -714,7 +813,9 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
             throw std::runtime_error(split_err);
         }
         const int n_dev = d->n_dev, n_host = nloc - n_dev;
-        // rows of the tensor from the rows Trows[nr][nas] of the metric transform into out[nr][npair] (zero-filled)
+        // rows of the tensor from the rows Trows[nr][nas] of the metric transform into out[nr][ncol] (zero-filled); under pair
+        // screening only the kept shell pairs are integrated and their columns written through col_of
+        const bool kept = d->pair_screened;
         auto fill_rows = [&](const double* Trows, int nr, double* out) {
             for_each_j3c_batch(h, d, omega, st, [&](int64_t col0, int64_t cols, const double* d_xa, int cb, int p0, int p1) {
                 if (nr <= 0) return;
@@ -733,10 +834,11 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
                     }
 #endif
                 const int la = h->pc[cb].la, lb = h->pc[cb].lb;
-                PairC2SBatchFn p2{d_ybatch, out, cols, col0, npair, h->pc[cb].d_all + p0, d->d_ao_off[cb] + p0, p1 - p0, la, lb,
-                                  h->d_sh_sph, h->d_c2s_off, h->d_c2s};
+                PairC2SBatchFn p2{d_ybatch, out, cols, col0, ncol, (kept ? d->d_kpairs[cb] : h->pc[cb].d_all) + p0,
+                                  (kept ? d->d_koff[cb] : d->d_ao_off[cb]) + p0, p1 - p0, la, lb, h->d_sh_sph, h->d_c2s_off, h->d_c2s,
+                                  d->d_col_of};
                 launch_1d((long)nr * (p1 - p0) * (2 * la + 1) * (2 * lb + 1), p2, st);
-            });
+            }, kept);
         };
         if (n_dev > 0 || n_host == 0) fill_rows(d_T, n_dev, d->d_cderi);
         if (n_host > 0) {
@@ -747,15 +849,15 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
             size_t freeb = 0, totb = 0;
             CK(cudaMemGetInfo(&freeb, &totb));
             const double scratch = (double)(d->naux_cart + nas) * bcols * 8 + (double)(1UL << 30);   // for_each_j3c_batch + margin
-            if ((double)freeb > scratch + npair * 8.0) hb = std::max(hb, (long)(((double)freeb - scratch) / (npair * 8.0)));
+            if ((double)freeb > scratch + ncol * 8.0) hb = std::max(hb, (long)(((double)freeb - scratch) / (ncol * 8.0)));
 #endif
             hb = std::max(1L, std::min<long>(hb, n_host));
-            double* d_blk = (double*)dev_alloc((size_t)hb * npair * 8);
+            double* d_blk = (double*)dev_alloc((size_t)hb * ncol * 8);
             for (int a = n_dev; a < nloc; a += (int)hb) {
                 const int nr = (int)std::min<long>(hb, nloc - a);
-                dev_zero(d_blk, (size_t)nr * npair * 8, st);
+                dev_zero(d_blk, (size_t)nr * ncol * 8, st);
                 fill_rows(d_T + (size_t)a * nas, nr, d_blk);
-                d2h(d->h_cderi + (size_t)(a - n_dev) * npair, d_blk, (size_t)nr * npair * 8, st);
+                d2h(d->h_cderi + (size_t)(a - n_dev) * ncol, d_blk, (size_t)nr * ncol * 8, st);
             }
 #ifndef B200JK_EMULATE
             CK(cudaStreamSynchronize(st));
@@ -970,6 +1072,7 @@ extern "C" int b200jk_df_set_cderi(b200jk_handle h, const double* cderi, int nau
         stream_t st = 0;
 #endif
         d->npair = (long)nao * (nao + 1) / 2;
+        d->ncol = d->npair;     // an assigned tensor stays dense: pair screening applies to tensors built here
         d->naux = naux;
         const int bw = h->shard_world, br = h->shard_rank;
         const int r_lo = (int)((long)naux * br / bw), r_hi = (int)((long)naux * (br + 1) / bw);
@@ -995,9 +1098,14 @@ extern "C" int b200jk_df_local_rows(b200jk_handle h, int* row0, int* nrow)
 
 // Columns cols[ncols] (packed AO-pair indices mu(mu+1)/2+nu) of all LOCAL rows: out[nrow][ncols] — what numpy slicing
 // dfobj._cderi[:, cols] gives on the reference's ndarray tensor (pyscf/df/df.py:116); samples a tensor too large to copy.
-struct GatherColsFn {
-    const double* cderi; const long* cols; double* out; long npair; int ncols;
-    B2_HD void operator()(long idx) const { long r = idx / ncols; int c = (int)(idx - r * ncols); out[idx] = cderi[r * npair + cols[c]]; }
+// Under pair screening a dropped column reads as exact zeros.
+struct GatherColsFn {   // cols: positions in the stored rows of length ld, -1 for a column that is not stored (0)
+    const double* cderi; const long* cols; double* out; long ld; int ncols;
+    B2_HD void operator()(long idx) const
+    {
+        long r = idx / ncols; int c = (int)(idx - r * ncols);
+        out[idx] = cols[c] >= 0 ? cderi[r * ld + cols[c]] : 0.0;
+    }
 };
 extern "C" int b200jk_df_get_cderi_cols(b200jk_handle h, double* out, const int64_t* cols, int ncols)
 {
@@ -1009,36 +1117,48 @@ extern "C" int b200jk_df_get_cderi_cols(b200jk_handle h, double* out, const int6
             if (cols[c] < 0 || cols[c] >= d->npair) throw std::runtime_error("column index out of range");
         if (d->nrow < 1) return 0;
         static_assert(sizeof(long) == sizeof(int64_t), "LP64");
+        std::vector<long> pos(cols, cols + ncols);     // positions in the stored rows
+        if (d->d_col_of)
+            for (long& p : pos) p = d->col_of_h[(size_t)p];
         if (d->n_dev > 0) {
             long* d_cols = (long*)dev_alloc((size_t)ncols * 8);
             double* d_out = (double*)dev_alloc((size_t)d->n_dev * ncols * 8);
-            h2d(d_cols, cols, (size_t)ncols * 8);
-            GatherColsFn g{d->d_cderi, d_cols, d_out, d->npair, ncols};
+            h2d(d_cols, pos.data(), (size_t)ncols * 8);
+            GatherColsFn g{d->d_cderi, d_cols, d_out, d->ncol, ncols};
             launch_1d((long)d->n_dev * ncols, g, 0);
             d2h(out, d_out, (size_t)d->n_dev * ncols * 8);
             dev_sync();
             dev_free(d_cols); dev_free(d_out);
         }
         for (long r = 0; r < d->nrow - d->n_dev; r++)      // rows in pinned host memory
-            for (int c = 0; c < ncols; c++) out[(d->n_dev + r) * ncols + c] = d->h_cderi[r * d->npair + cols[c]];
+            for (int c = 0; c < ncols; c++) out[(d->n_dev + r) * ncols + c] = pos[c] >= 0 ? d->h_cderi[r * d->ncol + pos[c]] : 0.0;
     } catch (std::exception& e) { set_err(h, e.what()); return 2; }
     return 0;
 }
 
-// cderi rows [r0, r0+nr) copied to the host (tests, interchange with PySCF's with_df._cderi)
+// cderi rows [r0, r0+nr) copied to the host in the reference layout [nr][nao(nao+1)/2] (tests, interchange with PySCF's
+// with_df._cderi); a pair-screened tensor is expanded, with exact zeros at the dropped columns
 extern "C" int b200jk_df_get_cderi(b200jk_handle h, double* out, int r0, int nr)
 {
     if (!h || !h->df || !h->df->d_cderi) { set_err(h, "call b200jk_df_build first"); return 1; }
     try {
         DFState* d = h->df;
         if (r0 < 0 || nr < 0 || r0 + nr > d->nrow) throw std::runtime_error("row range out of bounds (rows are local to this rank)");
+        const long ld = d->ncol;
+        std::vector<double> packed(d->d_col_of ? (size_t)nr * ld : 0);
+        double* dst = d->d_col_of ? packed.data() : out;    // the stored rows, expanded below when pair-screened
         const int nd = std::max(0, std::min(r0 + nr, d->n_dev) - r0);     // rows in HBM, then rows in pinned host memory
         if (nd > 0) {
-            d2h(out, d->d_cderi + (size_t)r0 * d->npair, (size_t)nd * d->npair * 8);
+            d2h(dst, d->d_cderi + (size_t)r0 * ld, (size_t)nd * ld * 8);
             dev_sync();
         }
         if (nr > nd)
-            memcpy(out + (size_t)nd * d->npair, d->h_cderi + (size_t)(r0 + nd - d->n_dev) * d->npair, (size_t)(nr - nd) * d->npair * 8);
+            memcpy(dst + (size_t)nd * ld, d->h_cderi + (size_t)(r0 + nd - d->n_dev) * ld, (size_t)(nr - nd) * ld * 8);
+        if (d->d_col_of) {
+            memset(out, 0, (size_t)nr * d->npair * 8);
+            for (long r = 0; r < nr; r++)
+                for (long c = 0; c < ld; c++) out[r * d->npair + d->pk_of_h[(size_t)c]] = packed[(size_t)(r * ld + c)];
+        }
     } catch (std::exception& e) { set_err(h, e.what()); return 2; }
     return 0;
 }
@@ -1054,6 +1174,9 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
         if (n_dm < 1) throw std::runtime_error("n_dm < 1");
         auto t0 = std::chrono::steady_clock::now();
         const long npair = d->npair, n2 = (long)nao * nao;
+        // row length of the stored tensor: npair, or the kept columns of a pair-screened tensor (col_of: packed index -> column)
+        const long ld = d->ncol;
+        const int* col_of = d->d_col_of;
         const int naux = std::max(d->nrow, 1);   // rows held locally
         // multi-GPU: this rank contracts only its auxiliary rows [r_lo, r_hi) and returns partial J/K
         int r_lo, r_hi;   // LOCAL row indices into d_cderi
@@ -1076,8 +1199,8 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
         if (d->kb_max > 0) kb = std::min(kb, d->kb_max);
         if ((size_t)n_dm > d->ws_ndm) {
             for (double** p : {&d->d_dmtril, &d->d_rho, &d->d_vjtril, &d->d_dm, &d->d_vk, &d->d_vj}) { dev_free(*p); *p = nullptr; }
-            d->d_dmtril = (double*)dev_alloc((size_t)n_dm * npair * 8);
-            d->d_vjtril = (double*)dev_alloc((size_t)n_dm * npair * 8);
+            d->d_dmtril = (double*)dev_alloc((size_t)n_dm * ld * 8);
+            d->d_vjtril = (double*)dev_alloc((size_t)n_dm * ld * 8);
             d->d_rho = (double*)dev_alloc((size_t)n_dm * naux * 8);
             d->d_dm = (double*)dev_alloc((size_t)n_dm * n2 * 8);
             d->d_vk = (double*)dev_alloc((size_t)n_dm * n2 * 8);
@@ -1123,7 +1246,7 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
             blk_rows(b, a, nr);
             if (b >= 2) CK(cudaStreamWaitEvent(d->cp_stream, d->ev_free[b & 1], 0));
             CK(cudaEventRecord(d->sx_ev[4 * b], d->cp_stream));
-            CK(cudaMemcpyAsync(d->d_stage[b & 1], d->h_cderi + (size_t)(a - d->n_dev) * npair, (size_t)nr * npair * 8,
+            CK(cudaMemcpyAsync(d->d_stage[b & 1], d->h_cderi + (size_t)(a - d->n_dev) * ld, (size_t)nr * ld * 8,
                                cudaMemcpyHostToDevice, d->cp_stream));
             CK(cudaEventRecord(d->sx_ev[4 * b + 1], d->cp_stream));
         };
@@ -1131,12 +1254,12 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
         auto issue_copy = [&](int b) {
             int a, nr;
             blk_rows(b, a, nr);
-            memcpy(d->d_stage[b & 1], d->h_cderi + (size_t)(a - d->n_dev) * npair, (size_t)nr * npair * 8);
+            memcpy(d->d_stage[b & 1], d->h_cderi + (size_t)(a - d->n_dev) * ld, (size_t)nr * ld * 8);
         };
 #endif
         for (int b = 0; b < std::min(nblk, 2); b++) issue_copy(b);
         auto finish_j = [&]() {
-            UnpackTrilFn uf{d->d_vjtril, d->d_vj, nao, npair};
+            UnpackTrilFn uf{d->d_vjtril, d->d_vj, nao, ld, col_of};     // a dropped pair gets J = 0
             launch_1d((long)n_dm * n2, uf, st); launches++;
             if (!on_device) d2h(vj, d->d_vj, (size_t)n_dm * n2 * 8, st);
             else {
@@ -1147,19 +1270,19 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
         };
 #ifndef B200JK_EMULATE
         const long seglen = 16384;   // 128 KiB of a row per CTA
-        const unsigned nseg = (unsigned)((npair + seglen - 1) / seglen);
+        const unsigned nseg = (unsigned)((ld + seglen - 1) / seglen);
         // J of the rows [r0, r0 + nr) at src (row r0 first): rho, then J~ += rho . rows
         auto j_rows = [&](const double* src, int r0, int nr) {
             mark(B200JK_DF_STAGE_J_RHO);
             for (int q = 0; q < nr; q += 32768 * DFJ_R) {
                 const int m = std::min(32768 * DFJ_R, nr - q);
-                dfj_rho_kernel<<<dim3(nseg, (m + DFJ_R - 1) / DFJ_R, n_dm), 256, 0, st>>>(src, d->d_dmtril, d->d_rho + r0, npair, q, q + m, naux, seglen, npair);
+                dfj_rho_kernel<<<dim3(nseg, (m + DFJ_R - 1) / DFJ_R, n_dm), 256, 0, st>>>(src, d->d_dmtril, d->d_rho + r0, ld, q, q + m, naux, seglen, ld);
                 launches++;
             }
             mark(B200JK_DF_STAGE_J_ACC);
-            const unsigned ncb = (unsigned)((npair + 255) / 256);
+            const unsigned ncb = (unsigned)((ld + 255) / 256);
             unsigned gy = (unsigned)std::max<long>(1, std::min<long>(nr / 64, (6L * device_sm_count() * 8 + ncb - 1) / ncb));
-            dfj_acc_kernel<<<dim3(ncb, gy), 256, 0, st>>>(src, d->d_rho + r0, d->d_vjtril, npair, 0, nr, naux, n_dm, npair);
+            dfj_acc_kernel<<<dim3(ncb, gy), 256, 0, st>>>(src, d->d_rho + r0, d->d_vjtril, ld, 0, nr, naux, n_dm, ld);
             launches++;
             mark(-1);
             CK(cudaGetLastError());
@@ -1169,21 +1292,21 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
             for (int s = 0; s < n_dm; s++)
                 for (int r = 0; r < nr; r++) {
                     double acc = 0;
-                    for (long t = 0; t < npair; t++) acc += src[(size_t)r * npair + t] * d->d_dmtril[(size_t)s * npair + t];
-                    for (long t = 0; t < npair; t++) d->d_vjtril[(size_t)s * npair + t] += acc * src[(size_t)r * npair + t];
+                    for (long t = 0; t < ld; t++) acc += src[(size_t)r * ld + t] * d->d_dmtril[(size_t)s * ld + t];
+                    for (long t = 0; t < ld; t++) d->d_vjtril[(size_t)s * ld + t] += acc * src[(size_t)r * ld + t];
                 }
         };
 #endif
         if (vj) {
-            DmTrilFn tf{d->d_dm, d->d_dmtril, nao, npair};
-            launch_1d((long)n_dm * npair, tf, st); launches++;
-            dev_zero(d->d_vjtril, (size_t)n_dm * npair * 8, st);
+            DmTrilFn tf{d->d_dm, d->d_dmtril, nao, ld, d->d_pk_of};     // pair screening: the kept columns only
+            launch_1d((long)n_dm * ld, tf, st); launches++;
+            dev_zero(d->d_vjtril, (size_t)n_dm * ld * 8, st);
 #ifndef B200JK_EMULATE
             dev_zero(d->d_rho, (size_t)n_dm * naux * 8, st);
 #endif
             // two streaming passes over the device rows (rho, then J): 2 launches, both HBM-bound
             (void)rb;
-            if (!streamed || r_dev > r_lo) j_rows(d->d_cderi + (size_t)r_lo * npair, r_lo, r_dev - r_lo);
+            if (!streamed || r_dev > r_lo) j_rows(d->d_cderi + (size_t)r_lo * ld, r_lo, r_dev - r_lo);
             if (!streamed) finish_j();
         }
         const bool use_occ = (occ != nullptr && nocc > 0);
@@ -1227,7 +1350,7 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
                     d->d_rownorm2 = (float*)dev_alloc((size_t)std::max(d->nrow, 1) * nao * 4);
                     d->d_cmax2 = (double*)dev_alloc(8);
                     if (d->n_dev == d->nrow || d->n_dev > 0)     // host rows: per staged block, every call
-                        i8g::packed_rowexp(d->d_cderi, npair, nao, d->n_dev, d->d_rowexp, d->d_rownorm2, st);
+                        i8g::packed_rowexp(d->d_cderi, ld, nao, d->n_dev, d->d_rowexp, d->d_rownorm2, st, col_of);
                 }
             }
 #endif
@@ -1254,7 +1377,7 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
                     d->SA.alloc((int)rows_p, nao, d->k_slices);
                     CK(cudaMemsetAsync(d->SA.q, 0, (size_t)d->k_slices * rp * kp, st));
                     CK(cudaMemsetAsync(d->SA.E, 0, rp * 4, st));
-                    i8g::split_packed_into(d->SA, 0, d->d_cderi + (size_t)r_lo * npair, npair, nao, (int)np, d->d_rowexp + (size_t)r_lo * nao, st);
+                    i8g::split_packed_into(d->SA, 0, d->d_cderi + (size_t)r_lo * ld, ld, nao, (int)np, d->d_rowexp + (size_t)r_lo * nao, st, col_of);
                 }
                 d->sa_decided = true; d->sa_ns = d->k_slices; d->sa_lo = r_lo; d->sa_hi = r_hi;
             }
@@ -1265,7 +1388,7 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
                 if (tc) {
                     if (!blk_resident) {    // slices of this block straight from the packed rows
                         mark(B200JK_DF_STAGE_K_SLICE);
-                        i8g::split_packed(d->SAt, src, npair, nao, nr, d->d_rowexp + (size_t)r0 * nao, d->k_slices, st);
+                        i8g::split_packed(d->SAt, src, ld, nao, nr, d->d_rowexp + (size_t)r0 * nao, d->k_slices, st, col_of);
                         mark(-1);
                         launches++;
                     }
@@ -1274,18 +1397,18 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
                         // same (P, k) column layout as Y: k padded to 16 when stage 1 cuts the slices of Y itself
                         static const bool fuse_y_g = getenv("B200JK_NO_YFUSE") == nullptr;
                         const int gcol = fuse_y_g ? ((nao + 15) & ~15) : nao;
-                        UnpackLongFn ul{src, d->d_A, nao, npair, 0, (long)nr * gcol, gcol};
+                        UnpackLongFn ul{src, d->d_A, nao, ld, 0, (long)nr * gcol, gcol, col_of};
                         launch_1d((long)nao * nr * gcol, ul, st);
                         i8g::split_rows(d->SG, d->d_A, (long)nr * gcol, nao, nr * gcol, d->k_slices, st);
                         mark(-1);
                         launches += 2;
                     }
                 } else {
-                    UnpackFn up{src, d->d_A, nao, npair, 0};
+                    UnpackFn up{src, d->d_A, nao, ld, 0, col_of};
                     launch_1d((long)nr * n2, up, st); launches++;
                 }
 #else
-                UnpackFn up{src, d->d_A, nao, npair, 0};
+                UnpackFn up{src, d->d_A, nao, ld, 0, col_of};
                 launch_1d((long)nr * n2, up, st); launches++;
 #endif
                 for (int s = 0; s < n_dm; s++) {
@@ -1409,7 +1532,7 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
 #endif
                 }
             };
-            for (int r0 = r_lo; r0 < r_dev; r0 += kb) k_block(d->d_cderi + (size_t)r0 * npair, r0, std::min(kb, r_dev - r0));
+            for (int r0 = r_lo; r0 < r_dev; r0 += kb) k_block(d->d_cderi + (size_t)r0 * ld, r0, std::min(kb, r_dev - r0));
         }
         if (streamed) {
             for (int b = 0; b < nblk; b++) {
@@ -1424,15 +1547,15 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
                 if (vj) j_rows(src, r0, nr);
                 if (vk) {
 #ifndef B200JK_EMULATE
-                    if (tc) { i8g::packed_rowexp(src, npair, nao, nr, d->d_rowexp + (size_t)r0 * nao, d->d_rownorm2 + (size_t)r0 * nao, st); launches++; }
+                    if (tc) { i8g::packed_rowexp(src, ld, nao, nr, d->d_rowexp + (size_t)r0 * nao, d->d_rownorm2 + (size_t)r0 * nao, st, col_of); launches++; }
 #endif
-                    for (int q = 0; q < nr; q += kb) k_block(src + (size_t)q * npair, r0 + q, std::min(kb, nr - q));
+                    for (int q = 0; q < nr; q += kb) k_block(src + (size_t)q * ld, r0 + q, std::min(kb, nr - q));
                 }
 #ifndef B200JK_EMULATE
                 CK(cudaEventRecord(d->ev_free[b & 1], st));
 #endif
                 if (b + 2 < nblk) issue_copy(b + 2);
-                d->stream_bytes += (int64_t)nr * npair * 8;
+                d->stream_bytes += (int64_t)nr * ld * 8;
             }
             if (vj) finish_j();
         }
@@ -1513,6 +1636,21 @@ extern "C" int b200jk_df_set_device_rows(b200jk_handle h, int max_rows)
     if (!h) return 1;
     if (max_rows < -1) { set_err(h, "bad device row cap"); return 1; }
     h->df_dev_rows = max_rows;
+    return 0;
+}
+
+extern "C" int b200jk_df_set_pair_tol(b200jk_handle h, double tol)
+{
+    if (!h) return 1;
+    if (std::isnan(tol)) { set_err(h, "bad pair tolerance"); return 1; }
+    h->df_pair_tol = tol > 0.0 ? tol : 0.0;
+    return 0;
+}
+
+extern "C" int b200jk_df_pair_stats(b200jk_handle h, int64_t* ncol, int64_t* npair)
+{
+    if (!h || !h->df || !ncol || !npair) { set_err(h, "call b200jk_df_build first"); return 1; }
+    *ncol = h->df->ncol; *npair = h->df->npair;
     return 0;
 }
 

@@ -100,17 +100,26 @@ void split_rows(SliceStack& S, const double* X, long ldx, int rows, int k, int n
 
 // ---- the DF tensor from its packed rows (see i8gemm.cuh (3)) ----
 // rowexp[nr][nao]: exponent of every row (P, a) of the unpacked tensor; cderi points at the first of the nr packed rows
-void packed_rowexp(const double* cderi, long npair, int nao, int nr, int* rowexp, float* rownorm2, cudaStream_t st)
+void packed_rowexp(const double* cderi, long npair, int nao, int nr, int* rowexp, float* rownorm2, cudaStream_t st, const int* col_of)
 {
     CK(cudaMemsetAsync(rowexp, 0x80, (size_t)nr * nao * 4, st));     // EXP_NONE
     if (rownorm2) CK(cudaMemsetAsync(rownorm2, 0, (size_t)nr * nao * 4, st));
     static bool configured = false;
-    if (!configured) { CK(cudaFuncSetAttribute(packed_rowexp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); configured = true; }
+    if (!configured) {
+        CK(cudaFuncSetAttribute(packed_rowexp_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+        CK(cudaFuncSetAttribute(packed_rowexp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+        configured = true;
+    }
     if ((size_t)nao * 8 > 160 * 1024) throw std::runtime_error("packed_rowexp: nao too large for the shared-memory tables");
     for (int p0 = 0; p0 < nr; p0 += 32768) {
         int n = std::min(32768, nr - p0);
-        packed_rowexp_kernel<<<dim3((nao + 63) / 64, n), 256, (size_t)nao * 8, st>>>(cderi + (size_t)p0 * npair, npair, nao, rowexp + (size_t)p0 * nao,
-                                                                                      rownorm2 ? rownorm2 + (size_t)p0 * nao : nullptr);
+        const dim3 grid((nao + 63) / 64, n);
+        if (col_of)
+            packed_rowexp_kernel<true><<<grid, 256, (size_t)nao * 8, st>>>(cderi + (size_t)p0 * npair, npair, nao, rowexp + (size_t)p0 * nao,
+                                                                           rownorm2 ? rownorm2 + (size_t)p0 * nao : nullptr, col_of);
+        else
+            packed_rowexp_kernel<false><<<grid, 256, (size_t)nao * 8, st>>>(cderi + (size_t)p0 * npair, npair, nao, rowexp + (size_t)p0 * nao,
+                                                                            rownorm2 ? rownorm2 + (size_t)p0 * nao : nullptr, nullptr);
     }
     CK(cudaGetLastError());
 }
@@ -139,24 +148,29 @@ void y_prepare(SliceStack& S, int nao, int nr, int ncolp, int ns, const float* r
     CK(cudaGetLastError());
 }
 // slices of the unpacked rows (P, a), P in [0, nr), into the rows out_row0 + P nao + a of an allocated stack
-void split_packed_into(SliceStack& S, int out_row0, const double* cderi, long npair, int nao, int nr, const int* rowexp, cudaStream_t st)
+void split_packed_into(SliceStack& S, int out_row0, const double* cderi, long npair, int nao, int nr, const int* rowexp, cudaStream_t st,
+                       const int* col_of)
 {
     if (S.K != nao) throw std::runtime_error("split_packed: stack width does not match nao");
     S.dmax = S.ns <= 7 ? 127 : 64;
     const unsigned nt = (unsigned)(S.Kp / PT);
     for (int p0 = 0; p0 < nr; p0 += 32768) {
         int n = std::min(32768, nr - p0);
-        if (S.ns == 7)
-            split_packed_kernel<true><<<dim3(nt, nt, n), 256, 0, st>>>(cderi + (size_t)p0 * npair, npair, nao, rowexp + (size_t)p0 * nao, S.ns, S.Rp, S.Kp,
-                                                                       out_row0 + p0 * nao, S.q, S.E);
-        else
-            split_packed_kernel<false><<<dim3(nt, nt, n), 256, 0, st>>>(cderi + (size_t)p0 * npair, npair, nao, rowexp + (size_t)p0 * nao, S.ns, S.Rp, S.Kp,
-                                                                        out_row0 + p0 * nao, S.q, S.E);
+        const dim3 grid(nt, nt, n);
+        const double* src = cderi + (size_t)p0 * npair;
+        const int* ex = rowexp + (size_t)p0 * nao;
+        if (S.ns == 7) {
+            if (col_of) split_packed_kernel<true, true><<<grid, 256, 0, st>>>(src, npair, nao, ex, S.ns, S.Rp, S.Kp, out_row0 + p0 * nao, S.q, S.E, col_of);
+            else split_packed_kernel<true, false><<<grid, 256, 0, st>>>(src, npair, nao, ex, S.ns, S.Rp, S.Kp, out_row0 + p0 * nao, S.q, S.E, nullptr);
+        } else {
+            if (col_of) split_packed_kernel<false, true><<<grid, 256, 0, st>>>(src, npair, nao, ex, S.ns, S.Rp, S.Kp, out_row0 + p0 * nao, S.q, S.E, col_of);
+            else split_packed_kernel<false, false><<<grid, 256, 0, st>>>(src, npair, nao, ex, S.ns, S.Rp, S.Kp, out_row0 + p0 * nao, S.q, S.E, nullptr);
+        }
     }
     CK(cudaGetLastError());
 }
 // a stack holding exactly these nr packed rows (allocated here, pad rows zeroed)
-void split_packed(SliceStack& S, const double* cderi, long npair, int nao, int nr, const int* rowexp, int ns, cudaStream_t st)
+void split_packed(SliceStack& S, const double* cderi, long npair, int nao, int nr, const int* rowexp, int ns, cudaStream_t st, const int* col_of)
 {
     const int rows = nr * nao;
     S.alloc(rows, nao, ns);
@@ -165,7 +179,7 @@ void split_packed(SliceStack& S, const double* cderi, long npair, int nao, int n
             CK(cudaMemsetAsync(S.q + ((size_t)s * S.Rp + rows) * S.Kp, 0, (size_t)(S.Rp - rows) * S.Kp, st));
         CK(cudaMemsetAsync(S.E + rows, 0, (size_t)(S.Rp - rows) * 4, st));
     }
-    split_packed_into(S, 0, cderi, npair, nao, nr, rowexp, st);
+    split_packed_into(S, 0, cderi, npair, nao, nr, rowexp, st, col_of);
 }
 
 static int sm_count()

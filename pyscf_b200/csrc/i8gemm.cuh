@@ -491,8 +491,21 @@ __device__ __forceinline__ int frexp_exp(double v)   // e with |v| = f 2^e, f in
 // counts for row a (warp reduction) and for row b (shared-memory atomicMax, flushed once per CTA).
 // rownorm2[P][a] (optional, zeroed by the caller) = sum_b A_P[a][b]^2 in single precision: the row norms behind the exponent
 // bound of Y when stage 1 cuts the slices of Y itself.
+// Pair-screened rows (MAP): a row of length npair holds only the kept packed columns; element t of the packed triangle is
+// row[col_of[t]], or 0 for col_of[t] < 0.  On the same values both variants give the same exponents, norms and digits.
+template <bool MAP>
+__device__ __forceinline__ double packed_load(const double* __restrict__ row, const int* __restrict__ col_of, long t)
+{
+    if constexpr (MAP) {
+        const int c = col_of[t];
+        return c >= 0 ? row[c] : 0.0;
+    } else {
+        return row[t];
+    }
+}
+template <bool MAP>
 __global__ void __launch_bounds__(256) packed_rowexp_kernel(const double* __restrict__ cderi, long npair, int nao, int* __restrict__ rowexp,
-                                                            float* __restrict__ rownorm2)
+                                                            float* __restrict__ rownorm2, const int* __restrict__ col_of)
 {
     extern __shared__ int emax_s[];          // [nao] exponents, then [nao] partial squared norms
     float* ss = reinterpret_cast<float*>(emax_s + nao);
@@ -503,11 +516,11 @@ __global__ void __launch_bounds__(256) packed_rowexp_kernel(const double* __rest
     __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     for (int a = a0 + warp; a < a1; a += 8) {
-        const double* x = row + (long)a * (a + 1) / 2;
+        const long ta = (long)a * (a + 1) / 2;
         int em = EXP_NONE;
         float sq = 0.0f;
         for (int b = lane; b <= a; b += 32) {
-            const double v = fabs(x[b]);
+            const double v = fabs(packed_load<MAP>(row, col_of, ta + b));
             if (v > 0.0) {
                 const int e = frexp_exp(v);
                 em = e > em ? e : em;
@@ -564,10 +577,11 @@ constexpr int PT = 64;   // tile edge of split_packed_kernel
 // (P, a) at columns b and — for off-diagonal tiles — the slices of the transposed tile to the rows (P, b) at columns a,
 // four int8 per 32-bit store.  Columns nao..Kp-1 are written as zeros; pad ROWS of the stack are the caller's (memset).
 // NS7: the slice count is the compile-time 7 (constant shift amounts, digits 3..6 from the low word, 0..1 from the high word)
-template <bool NS7>
+// MAP: pair-screened rows read through col_of (packed_load)
+template <bool NS7, bool MAP>
 __global__ void __launch_bounds__(256) split_packed_kernel(const double* __restrict__ cderi, long npair, int nao,
                                                            const int* __restrict__ rowexp, int ns, int Rp, int Kp, int out_row0,
-                                                           int8_t* __restrict__ out, int* __restrict__ E)
+                                                           int8_t* __restrict__ out, int* __restrict__ E, const int* __restrict__ col_of)
 {
     const int ta = blockIdx.x, tb = blockIdx.y, P = blockIdx.z;
     if (tb > ta) return;
@@ -580,7 +594,7 @@ __global__ void __launch_bounds__(256) split_packed_kernel(const double* __restr
         const int idx = t + 256 * i, al = idx >> 6, bl = idx & 63;
         const int a = ta * PT + al, b = tb * PT + bl;
         double v = 0.0;
-        if (a < nao && b < nao) { const int hi = a > b ? a : b, lo = a > b ? b : a; v = row[(long)hi * (hi + 1) / 2 + lo]; }
+        if (a < nao && b < nao) { const int hi = a > b ? a : b, lo = a > b ? b : a; v = packed_load<MAP>(row, col_of, (long)hi * (hi + 1) / 2 + lo); }
         S[al][bl] = v;
     }
     __syncthreads();

@@ -18,11 +18,16 @@ void split_rows(SliceStack& S, const double* X, long ldx, int rows, int k, int n
 void split_rows_into(SliceStack& S, int row0, const double* X, long ldx, int rows, cudaStream_t st);
 // the DF tensor straight from its packed rows cderi[P][a(a+1)/2+b] (no fp64 unpacked copy): per-row exponents of the unpacked
 // rows (P, a), then their int8 slices
-void packed_rowexp(const double* cderi, long npair, int nao, int nr, int* rowexp, float* rownorm2, cudaStream_t st);
+// Packed DF rows of length npair; with col_of (pair-screened rows, i8gemm.cuh (3)) element t of the packed triangle is column
+// col_of[t] of the row, or 0 when col_of[t] < 0.
+void packed_rowexp(const double* cderi, long npair, int nao, int nr, int* rowexp, float* rownorm2, cudaStream_t st,
+                   const int* col_of = nullptr);
 void colnorm_max(const double* X, long ldx, int nrows, int k, double* cmax2, cudaStream_t st);
 void y_prepare(SliceStack& S, int nao, int nr, int ncolp, int ns, const float* rownorm2_block, const double* cmax2, cudaStream_t st);
-void split_packed_into(SliceStack& S, int out_row0, const double* cderi, long npair, int nao, int nr, const int* rowexp, cudaStream_t st);
-void split_packed(SliceStack& S, const double* cderi, long npair, int nao, int nr, const int* rowexp, int ns, cudaStream_t st);
+void split_packed_into(SliceStack& S, int out_row0, const double* cderi, long npair, int nao, int nr, const int* rowexp, cudaStream_t st,
+                       const int* col_of = nullptr);
+void split_packed(SliceStack& S, const double* cderi, long npair, int nao, int nr, const int* rowexp, int ns, cudaStream_t st,
+                  const int* col_of = nullptr);
 // Yout != nullptr: stage 1 writes the int8 slices of Y (columns (P, i), i padded to y_ncolp) instead of fp64 C
 void gemm_ar(const SliceStack& A, int a_row0, int M, const SliceStack& B, double* C, long ldc, int inner, cudaStream_t st,
              unsigned long long* rowmax = nullptr, const SliceStack* Yout = nullptr, int y_ncolp = 0);

@@ -9,6 +9,8 @@ Mirrors (names, argument meaning, shapes):
 The three-index tensor is built on the GPU (Rys kernels + cuSOLVER/cuBLAS for the metric) and stays
 resident in HBM in the reference layout cderi[naux, nao(nao+1)/2]; the rows of a tensor larger than the GPU that do not fit
 live in pinned host memory and are streamed through the GPU once per J/K call (set_device_rows, row_split).
+With pair_tol (opt-in, no reference equivalent) the tensor stores only the AO-pair columns whose Schwarz bound is >= pair_tol
+(pair_stats); loop(), cderi_columns(), save() and _cderi still return the reference layout, exact zeros at dropped columns.
 """
 import ctypes
 
@@ -19,7 +21,7 @@ from .gto.mole import make_auxmol
 
 
 class DF:
-    def __init__(self, mol, auxbasis=None, device=0, libpath=None, shard=None):
+    def __init__(self, mol, auxbasis=None, device=0, libpath=None, shard=None, pair_tol=None):
         self.mol = mol
         self.auxbasis = auxbasis
         self.auxmol = None
@@ -36,6 +38,9 @@ class DF:
         self.k_engine = 'tcgen05'
         self.k_slices = 7
         self.device_rows = -1      # cap on the tensor rows kept in HBM, the rest in pinned host memory (-1: automatic)
+        # pair screening: keep only the AO-pair columns whose shell-pair Schwarz bound sqrt((ab|ab)) is >= pair_tol (None: dense,
+        # the reference's tensor).  A dropped column has 2-norm < pair_tol.  Applies to built tensors, not to an assigned _cderi.
+        self.pair_tol = pair_tol
         self.verbose = getattr(mol, 'verbose', 0)
         self.stdout = getattr(mol, 'stdout', None)
         self.max_memory = getattr(mol, 'max_memory', 4000)
@@ -58,6 +63,7 @@ class DF:
             h.check(h.lib.b200jk_set_shard(h._h, int(self.shard[0]), int(self.shard[1])), 'b200jk_set_shard')
         self._built_omega = omega
         h.check(h.lib.b200jk_df_set_device_rows(h._h, int(self.device_rows)), 'b200jk_df_set_device_rows')
+        h.check(h.lib.b200jk_df_set_pair_tol(h._h, float(self.pair_tol or 0.0)), 'b200jk_df_set_pair_tol')
         h.check(h.lib.b200jk_df_build(h._h, _lib.iptr(atm), len(atm), _lib.iptr(bas), len(bas), _lib.dptr(env), len(env),
                                       omega, self.lindep), 'b200jk_df_build')
         self._handle = h
@@ -123,6 +129,14 @@ class DF:
         n_dev, n_host = ctypes.c_int(0), ctypes.c_int(0)
         h.check(h.lib.b200jk_df_row_split(h._h, ctypes.byref(n_dev), ctypes.byref(n_host)), 'b200jk_df_row_split')
         return n_dev.value, n_host.value
+
+    def pair_stats(self):
+        """(kept AO-pair columns, nao(nao+1)/2) of the tensor; equal without pair screening."""
+        self.get_naoaux()
+        h = self._handle
+        ncol, npair = ctypes.c_int64(0), ctypes.c_int64(0)
+        h.check(h.lib.b200jk_df_pair_stats(h._h, ctypes.byref(ncol), ctypes.byref(npair)), 'b200jk_df_pair_stats')
+        return ncol.value, npair.value
 
     def stream_stats(self):
         """Host rows streamed by the last get_jk: {'bytes', 'copy_ms', 'exposed_ms'} (exposed: copy time not hidden
@@ -206,6 +220,7 @@ class DF:
             rsh.lindep = self.lindep
             rsh.k_engine, rsh.k_slices = self.k_engine, self.k_slices
             rsh.device_rows = self.device_rows
+            rsh.pair_tol = self.pair_tol       # screened with the bound of its own operator
             self._rsh_df[key] = rsh.build()
         return self._rsh_df[key]
 

@@ -44,7 +44,8 @@ SYMBOLS = ['b200jk_create', 'b200jk_create2', 'b200jk_destroy', 'b200jk_set_scre
            'b200jk_set_profile', 'b200jk_get_class_times', 'b200jk_df_get_cderi', 'b200jk_i8gemm_test', 'b200jk_i8engine_test', 'b200jk_df_set_kmode', 'b200jk_df_set_kblock', 'b200jk_set_shard', 'b200jk_df_jk_device', 'b200jk_df_local_rows',
            'b200jk_df_prepare_j', 'b200jk_df_direct_j', 'b200jk_df_stage_times', 'b200jk_df_set_cderi', 'b200jk_df_get_cderi_cols',
            'b200jk_incore_set_eri', 'b200jk_incore_jk', 'b200jk_set_class_costs',
-           'b200jk_df_set_device_rows', 'b200jk_df_row_split', 'b200jk_df_stream_stats']
+           'b200jk_df_set_device_rows', 'b200jk_df_row_split', 'b200jk_df_stream_stats',
+           'b200jk_df_set_pair_tol', 'b200jk_df_pair_stats']
 
 
 def load(path=None):
@@ -87,6 +88,8 @@ def load(path=None):
     lib.b200jk_df_set_device_rows.argtypes = [vp, ctypes.c_int]
     lib.b200jk_df_row_split.argtypes = [vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]
     lib.b200jk_df_stream_stats.argtypes = [vp, ctypes.POINTER(ctypes.c_int64), c_double_p, c_double_p]
+    lib.b200jk_df_set_pair_tol.argtypes = [vp, ctypes.c_double]
+    lib.b200jk_df_pair_stats.argtypes = [vp, ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(ctypes.c_int64)]
     lib.b200jk_df_local_rows.argtypes = [vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]
     lib.b200jk_set_shard.argtypes = [vp, ctypes.c_int, ctypes.c_int]
     lib.b200jk_df_jk_device.argtypes = [vp, vp, ctypes.c_int, ctypes.c_int, vp, ctypes.c_int, ctypes.c_int, vp, vp]
