@@ -55,7 +55,8 @@ typedef struct {
 int b200jk_create(b200jk_handle* out, const int32_t* atm, int natm, const int32_t* bas, int nbas, const double* env,
                   int nenv, int device);
 /* The same with Cartesian AOs when cart != 0 (mol.cart = True; libcint's int2e_cart, pyscf/gto/moleintor.py:772): every dm / vj /
- * vk then runs over the (l+1)(l+2)/2 Cartesian functions of each shell.  4-center and in-core paths only (DF raises). */
+ * vk then runs over the (l+1)(l+2)/2 Cartesian functions of each shell.  Serves the 4-center, in-core and density-fitting paths;
+ * a DF tensor of such a handle is built in a Cartesian auxiliary basis (see b200jk_df_build). */
 int b200jk_create2(b200jk_handle* out, const int32_t* atm, int natm, const int32_t* bas, int nbas, const double* env,
                    int nenv, int device, int cart);
 int b200jk_destroy(b200jk_handle h);
@@ -79,7 +80,10 @@ int b200jk_direct_jk_device(b200jk_handle h, const double* dm_dev, int n_dm, int
 int b200jk_incore_set_eri(b200jk_handle h, const double* eri, int64_t neri, int nao);
 int b200jk_incore_jk(b200jk_handle h, const double* dm, int n_dm, int nao, double* vj, double* vk);
 
-/* Density fitting: aux tables are a second libcint-layout set for the auxiliary basis. */
+/* Density fitting: aux tables are a second libcint-layout set for the auxiliary basis.  The auxiliary functions follow the
+ * handle's AO convention, as the reference's make_auxmol copies mol.cart (pyscf/df/addons.py:245, incore.py:144-149): a
+ * Cartesian handle (b200jk_create2 with cart != 0) builds cderi[naux_cart][ncart(ncart+1)/2] from int3c2e_cart / int2c2e_cart,
+ * naux_cart counting (l+1)(l+2)/2 functions per auxiliary shell.  Mixing conventions is the caller's to refuse. */
 int b200jk_df_build(b200jk_handle h, const int32_t* aux_atm, int aux_natm, const int32_t* aux_bas, int aux_nbas,
                     const double* aux_env, int aux_nenv, double omega, double lindep);
 /* Integral-direct DF-J (df_jk.get_j, pyscf/df/df_jk.py:415-506; what DF.get_jk does for with_k=False while no tensor

@@ -200,6 +200,32 @@ struct PairC2SBatchFn {
     }
 };
 
+// The same scatter for a Cartesian handle (mol.cart = True): the AO functions are the Cartesian components themselves, so each
+// output element is one scaled copy, fab * X[b*nca + a] with fab = fac(la) fac(lb) the s/p factors of make_c2c.  One thread per
+// (row, pair, a, b); sh_sph holds the Cartesian AO offset of each device shell in the reference's order.
+struct PairCartBatchFn {
+    const double* in; double* out; int64_t cols, col0; long npair;
+    const ShellPair* pairs; const int64_t* off; int np; int la, lb; double fab;
+    const int* sh_sph;
+    const int* col_of;
+    B2_HD void operator()(long idx) const
+    {
+        const int nca = (la + 1) * (la + 2) / 2, ncb = (lb + 1) * (lb + 2) / 2;
+        const long per_row = (long)np * nca * ncb;
+        const long r = idx / per_row;
+        long e = idx - r * per_row;
+        const int p = (int)(e / (nca * ncb));
+        e -= (long)p * nca * ncb;
+        const int a = (int)(e / ncb), b = (int)(e - (long)a * ncb);
+        const ShellPair& sp = pairs[p];
+        const long mu = sh_sph[sp.ish] + a, nu = sh_sph[sp.jsh] + b;
+        if (sp.ish == sp.jsh && mu < nu) return;
+        const long hi = mu >= nu ? mu : nu, lo = mu >= nu ? nu : mu;
+        const long t = hi * (hi + 1) / 2 + lo;
+        out[r * npair + (col_of ? (long)col_of[t] : t)] = fab * in[r * cols + (off[p] - col0) + b * nca + a];
+    }
+};
+
 // dmtril[s][t] = D[mu,nu] + D[nu,mu] (diagonal once)      <- pyscf/df/df_jk.py:329-332
 // npair is the row length of out; with pair screening (pk_of != nullptr) column c holds the packed element pk_of[c]
 struct DmTrilFn {
@@ -371,6 +397,12 @@ static void cols_acc(const double* M, long nrow, long ncol, const double* x, int
 }
 #endif
 
+// functions per shell in the handle's AO convention: 2l+1 real spherical harmonics, or the ncart(l) Cartesian components of a
+// Cartesian handle (the auxiliary basis follows the same convention, as the reference's make_auxmol copies mol.cart)
+static int nfun(b200jk_handle h, int l) { return h->cart ? ncart(l) : 2 * l + 1; }
+
+// Auxiliary tables: for a Cartesian handle the "spherical" auxiliary index (naux_sph, d_asph_*) is the Cartesian one in the
+// reference's order, and h->d_c2s holds the make_c2c tables, so AuxC2SFn / Cart2SphFn reduce to the s/p factors.
 void build_aux(b200jk_handle h, DFState* d, const int32_t* atm, const int32_t* bas, int nbas, const double* env)
 {
     std::vector<DevShell> tmp;
@@ -382,7 +414,7 @@ void build_aux(b200jk_handle h, DFState* d, const int32_t* atm, const int32_t* b
         const double* r = env + atm[b[ATOM_OF] * ATM_SLOTS + PTR_COORD];
         for (int c = 0; c < nc; c++) {
             DevShell s;
-            s.l = l; s.ref_shell = ib; s.sph_off = sph + c * (2 * l + 1); s.cart_off = 0;
+            s.l = l; s.ref_shell = ib; s.sph_off = sph + c * nfun(h, l); s.cart_off = 0;
             s.r[0] = r[0]; s.r[1] = r[1]; s.r[2] = r[2];
             for (int p = 0; p < np; p++) {
                 double cf = env[b[PTR_COEFF] + c * np + p];
@@ -391,7 +423,7 @@ void build_aux(b200jk_handle h, DFState* d, const int32_t* atm, const int32_t* b
             s.nprim = (int)s.e.size();
             tmp.push_back(s);
         }
-        sph += nc * (2 * l + 1);
+        sph += nc * nfun(h, l);
     }
     d->naux_sph = sph;
     std::stable_sort(tmp.begin(), tmp.end(), [](const DevShell& a, const DevShell& b) { return a.l < b.l; });
@@ -406,7 +438,7 @@ void build_aux(b200jk_handle h, DFState* d, const int32_t* atm, const int32_t* b
         const DevShell& s = d->ash[i];
         sh_l[i] = s.l; sh_cart[i] = s.cart_off; sh_sph[i] = s.sph_off;
         for (int a = 0; a < ncart(s.l); a++) { cart_sh[s.cart_off + a] = i; cart_comp[s.cart_off + a] = a; }
-        for (int m = 0; m < 2 * s.l + 1; m++) { sph_sh[s.sph_off + m] = i; sph_m[s.sph_off + m] = m; }
+        for (int m = 0; m < nfun(h, s.l); m++) { sph_sh[s.sph_off + m] = i; sph_m[s.sph_off + m] = m; }
         ShellPair sp{};
         sp.ish = i; sp.jsh = -1; sp.i0 = s.cart_off; sp.j0 = 0; sp.same = 0;
         sp.prim_off = (int)d->aprims.size(); sp.nprim = s.nprim;
@@ -424,7 +456,6 @@ void build_aux(b200jk_handle h, DFState* d, const int32_t* atm, const int32_t* b
     for (int l = 0; l <= LMAX; l++) { d->d_akets[l] = upload(d->akets[l]); d->d_aket_off[l] = upload(koff[l]); }
     d->d_acart_sh = upload(cart_sh); d->d_acart_comp = upload(cart_comp); d->d_asph_sh = upload(sph_sh); d->d_asph_m = upload(sph_m);
     d->d_ash_l = upload(sh_l); d->d_ash_cart = upload(sh_cart); d->d_ash_sph = upload(sh_sph);
-    (void)h;
 }
 
 #ifdef B200JK_EMULATE
@@ -585,7 +616,7 @@ static void select_pairs(b200jk_handle h, DFState* d, double omega, double tol, 
             for (long i0 = 0; i0 < (long)pairs.size(); i0 += chunk) {
                 const long n = std::min<long>(chunk, (long)pairs.size() - i0);
                 SchwarzSphFn fn{d_tmp + i0, h->d_prims, h->tb, omega, P.la, P.lb, h->d_c2s + h->c2s_off[P.la], h->d_c2s + h->c2s_off[P.lb],
-                                scratch, 2 * P.la + 1, 2 * P.lb + 1};
+                                scratch, nfun(h, P.la), nfun(h, P.lb)};
                 launch_1d(n, fn, st);
 #ifndef B200JK_EMULATE
                 CK(cudaStreamSynchronize(st));
@@ -604,8 +635,8 @@ static void select_pairs(b200jk_handle h, DFState* d, double omega, double tol, 
             koff.push_back(off);
             off += ncart(P.la) * ncart(P.lb);
             const DevShell &a = h->sh[sp.ish], &b = h->sh[sp.jsh];
-            for (int ma = 0; ma < 2 * a.l + 1; ma++)
-                for (int mb = 0; mb < 2 * b.l + 1; mb++) {
+            for (int ma = 0; ma < nfun(h, a.l); ma++)
+                for (int mb = 0; mb < nfun(h, b.l); mb++) {
                     const long mu = a.sph_off + ma, nu = b.sph_off + mb;
                     if (sp.ish == sp.jsh && mu < nu) continue;
                     const long hi = std::max(mu, nu), lo = std::min(mu, nu);
@@ -633,7 +664,6 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
 {
     if (!h) return 1;
     try {
-        if (h->cart) throw std::runtime_error("density fitting with Cartesian AOs (mol.cart = True) is not supported");
         (void)aux_natm; (void)aux_nenv;
         if (h->df) { df_free(h->df); h->df = nullptr; }
         DFState* d = new DFState();
@@ -834,10 +864,17 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
                     }
 #endif
                 const int la = h->pc[cb].la, lb = h->pc[cb].lb;
-                PairC2SBatchFn p2{d_ybatch, out, cols, col0, ncol, (kept ? d->d_kpairs[cb] : h->pc[cb].d_all) + p0,
-                                  (kept ? d->d_koff[cb] : d->d_ao_off[cb]) + p0, p1 - p0, la, lb, h->d_sh_sph, h->d_c2s_off, h->d_c2s,
-                                  d->d_col_of};
-                launch_1d((long)nr * (p1 - p0) * (2 * la + 1) * (2 * lb + 1), p2, st);
+                const ShellPair* bpairs = (kept ? d->d_kpairs[cb] : h->pc[cb].d_all) + p0;
+                const int64_t* boff = (kept ? d->d_koff[cb] : d->d_ao_off[cb]) + p0;
+                if (h->cart) {
+                    PairCartBatchFn p2{d_ybatch, out, cols, col0, ncol, bpairs, boff, p1 - p0, la, lb,
+                                       make_c2c(la)[0] * make_c2c(lb)[0], h->d_sh_sph, d->d_col_of};
+                    launch_1d((long)nr * (p1 - p0) * ncart(la) * ncart(lb), p2, st);
+                } else {
+                    PairC2SBatchFn p2{d_ybatch, out, cols, col0, ncol, bpairs, boff, p1 - p0, la, lb, h->d_sh_sph, h->d_c2s_off, h->d_c2s,
+                                      d->d_col_of};
+                    launch_1d((long)nr * (p1 - p0) * (2 * la + 1) * (2 * lb + 1), p2, st);
+                }
             }, kept);
         };
         if (n_dev > 0 || n_host == 0) fill_rows(d_T, n_dev, d->d_cderi);
@@ -945,7 +982,7 @@ extern "C" int b200jk_df_direct_j(b200jk_handle h, const double* dm, int n_dm, i
         double* d_dc = (double*)dev_alloc((size_t)d->rowlen * n_dm * 8);
         double* d_rho = (double*)dev_alloc((size_t)nas * n_dm * 8);
         h2d(d_dsph, dm, ns2 * n_dm * 8, st);
-        Sph2CartFn s2c{d_dsph, d_dcart, ns, nc, 0, h->d_cart_sh, h->d_cart_comp, h->d_sh_l, h->d_sh_sph, h->d_c2s_off, h->d_c2s};
+        Sph2CartFn s2c{d_dsph, d_dcart, ns, nc, 0, h->d_cart_sh, h->d_cart_comp, h->d_sh_l, h->d_sh_sph, h->d_c2s_off, h->d_c2s, h->cart};
         launch_1d((long)nc2 * n_dm, s2c, st);
         for (int cb = 0; cb < NPC; cb++) {
             const int np = (int)h->pc[cb].all.size();

@@ -9,6 +9,8 @@ Mirrors (names, argument meaning, shapes):
 The three-index tensor is built on the GPU (Rys kernels + cuSOLVER/cuBLAS for the metric) and stays
 resident in HBM in the reference layout cderi[naux, nao(nao+1)/2]; the rows of a tensor larger than the GPU that do not fit
 live in pinned host memory and are streamed through the GPU once per J/K call (set_device_rows, row_split).
+A Cartesian molecule (mol.cart = True) gets a Cartesian tensor [naux_cart, ncart(ncart+1)/2] in a Cartesian auxiliary basis, as
+the reference's make_auxmol / cholesky_eri give it (pyscf/df/addons.py:245, pyscf/df/incore.py:144-149).
 With pair_tol (opt-in, no reference equivalent) the tensor stores only the AO-pair columns whose Schwarz bound is >= pair_tol
 (pair_stats); loop(), cderi_columns(), save() and _cderi still return the reference layout, exact zeros at dropped columns.
 """
@@ -18,6 +20,24 @@ import numpy as np
 
 from . import lib as _lib
 from .gto.mole import make_auxmol
+
+
+def _is_cart(mol):
+    return bool(getattr(mol, 'cart', False))
+
+
+def _nao(mol):
+    """AO count in the molecule's own convention: (l+1)(l+2)/2 functions per shell when mol.cart, else 2l+1."""
+    return int(mol.ao_loc_nr(cart=_is_cart(mol))[-1])
+
+
+def _check_aux_cart(mol, auxmol):
+    """The tensor's auxiliary functions follow the AO convention; a user-assigned auxmol of the other one is refused with the
+    reference's messages (pyscf/df/incore.py:144-147)."""
+    if not _is_cart(mol) and _is_cart(auxmol):
+        raise NotImplementedError('Interface for int3c2e_ssc')
+    if _is_cart(mol) and not _is_cart(auxmol):
+        raise RuntimeError('Cartesian orbitals for mol and spherical orbitals for auxmol not supported')
 
 
 class DF:
@@ -53,8 +73,9 @@ class DF:
         if self.auxmol is None:
             self.auxmol = make_auxmol(mol, self.auxbasis)
         aux = self.auxmol
+        _check_aux_cart(mol, aux)
         h = _lib.Handle(mol._atm, mol._bas, np.array(mol._env, dtype=np.float64), device=self.device,
-                        libpath=self._libpath)
+                        libpath=self._libpath, cart=_is_cart(mol))
         atm = np.ascontiguousarray(aux._atm, dtype=np.int32)
         bas = np.ascontiguousarray(aux._bas, dtype=np.int32)
         env = np.ascontiguousarray(aux._env, dtype=np.float64)
@@ -67,7 +88,7 @@ class DF:
         h.check(h.lib.b200jk_df_build(h._h, _lib.iptr(atm), len(atm), _lib.iptr(bas), len(bas), _lib.dptr(env), len(env),
                                       omega, self.lindep), 'b200jk_df_build')
         self._handle = h
-        self.nao = int(mol.ao_loc_nr(cart=False)[-1])
+        self.nao = _nao(mol)
         self.set_k_engine(self.k_engine, self.k_slices)
         return self
 
@@ -86,12 +107,13 @@ class DF:
         c = self._cderi_in
         if isinstance(c, str):
             c = np.load(c, mmap_mode='r')
-        nao = int(mol.ao_loc_nr(cart=False)[-1])
+        nao = _nao(mol)
         npair = nao * (nao + 1) // 2
         if c.ndim != 2 or c.shape[1] != npair:
             raise RuntimeError('cderi must have shape (naux, nao*(nao+1)/2) = (*, %d), got %s' % (npair, c.shape))
         c = np.ascontiguousarray(c, dtype=np.float64)
-        h = _lib.Handle(mol._atm, mol._bas, np.array(mol._env, dtype=np.float64), device=self.device, libpath=self._libpath)
+        h = _lib.Handle(mol._atm, mol._bas, np.array(mol._env, dtype=np.float64), device=self.device, libpath=self._libpath,
+                        cart=_is_cart(mol))
         if self.shard is not None:
             h.check(h.lib.b200jk_set_shard(h._h, int(self.shard[0]), int(self.shard[1])), 'b200jk_set_shard')
         h.check(h.lib.b200jk_df_set_device_rows(h._h, int(self.device_rows)), 'b200jk_df_set_device_rows')
@@ -231,8 +253,9 @@ class DF:
         if self.auxmol is None:
             self.auxmol = make_auxmol(mol, self.auxbasis)
         aux = self.auxmol
+        _check_aux_cart(mol, aux)
         h = _lib.Handle(mol._atm, mol._bas, np.array(mol._env, dtype=np.float64), device=self.device,
-                        libpath=self._libpath)
+                        libpath=self._libpath, cart=_is_cart(mol))
         atm = np.ascontiguousarray(aux._atm, dtype=np.int32)
         bas = np.ascontiguousarray(aux._bas, dtype=np.int32)
         env = np.ascontiguousarray(aux._env, dtype=np.float64)
@@ -241,7 +264,7 @@ class DF:
         h.check(h.lib.b200jk_df_prepare_j(h._h, _lib.iptr(atm), len(atm), _lib.iptr(bas), len(bas), _lib.dptr(env),
                                           len(env), omega, self.lindep), 'b200jk_df_prepare_j')
         self._vjopt = h
-        self.nao = int(mol.ao_loc_nr(cart=False)[-1])
+        self.nao = _nao(mol)
         return h
 
     def get_j(self, dm, hermi=0, direct_scf_tol=1e-13):

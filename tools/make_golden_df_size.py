@@ -14,7 +14,11 @@ column, and J/K of a density SUPPORTED ON A FEW SHELLS S only need the slab (P|s
         J[s,nu] = sum_P B[P,s,nu] rho_P,  rho_P = sum_{j,k in S} B[P,j,k] D_S[j,k]    the rows s in S of J
     stored as `vk_idx`/`vk_val` (sampled elements), fp(K), and the J rows.  Both K engines (int8 slices on the
     orbital tag, FP64 general path on the bare matrix) are compared with these on the GPU (tests/test_df_size.py, bench.py).
-Usage: python tools/make_golden_df_size.py [c60 taxol taxol_svp gly30 gly30_lr]
+Cartesian cases (name in CART, mol.cart = True) take their integrals from tests/cart_oracle.py, the oracle library's Cartesian
+entry points, and also report the metric's condition number and the spread of the slab J/K when the 3-center and metric
+integrals carry 1e-15 relative noise: how well the Cartesian problem itself defines J/K (Cartesian auxiliary bases are much
+worse conditioned than spherical ones), which sets the bar of the GPU comparison.
+Usage: python tools/make_golden_df_size.py [c60 taxol taxol_svp gly30 gly30_lr c60_cart]
 """
 import os
 import sys
@@ -36,9 +40,12 @@ CASES = {   # name: (geometry, basis, nocc, omega)
     'gly30': ('gly30', 'cc-pvdz', 455, None),
     'gly30_lr': ('gly30', 'cc-pvdz', 455, 0.3),
     'gly4': ('gly4', 'cc-pvdz', 65, None),          # small: the same fixture at a size the CPU tests can build in full
+    'c60_cart': ('c60', 'cc-pvdz', 180, None),      # Cartesian AOs and auxiliary functions: nao 900, naux 4860
 }
+CART = {'c60_cart'}
+NOISE = 1e-15         # relative noise of the integrals in the conditioning probe of the Cartesian cases
 # fixtures kept below 1 MB: one shell pair per angular-momentum pair type, two components each, fewer sampled K elements
-SMALL = {'taxol_svp'}
+SMALL = {'taxol_svp', 'c60_cart'}
 
 
 def slab_coeff(nao, nocc, sao, seed=7):
@@ -94,22 +101,57 @@ def pick_slab_shells(mol, rng):
     return sorted(set(shells))
 
 
+def slab_jk(B, S, c0, mol, loc, sao, d_ss):
+    """J rows of the slab AOs and all of K for the density D_SS on the slab AOs, from the slab tensor B[P, (s, nu) blocks]."""
+    naux, nao = B.shape[0], int(loc[-1])
+    Bs = np.empty((naux, len(sao), nao))                       # reorder to B[P, s_ao, nu]
+    row = 0
+    for si, s in enumerate(S):
+        ds = loc[s + 1] - loc[s]
+        for j in range(mol.nbas):
+            p = si * mol.nbas + j
+            dj = loc[j + 1] - loc[j]
+            Bs[:, row:row + ds, loc[j]:loc[j + 1]] = B[:, c0[p]:c0[p] + ds * dj].reshape(naux, ds, dj)
+        row += ds
+    rho = np.einsum('psk,sk->p', Bs[:, :, sao], d_ss)
+    vj_rows = np.einsum('p,psn->sn', rho, Bs)                  # J[s, :] for s in sao
+    vk = np.zeros((nao, nao))
+    blk = 256
+    for p0 in range(0, naux, blk):
+        b = Bs[p0:p0 + blk]                                    # [pb, ns, nao]
+        t = np.matmul(d_ss, b)                                 # D_SS B_P[S,:]   [pb, ns, nao]
+        vk += b.reshape(-1, nao).T.dot(t.reshape(-1, nao))     # sum_{P,s} B[P,s,i] T[P,s,n]  (BLAS)
+    return vj_rows, vk
+
+
 def main(name):
     geom, basis, nocc, omega = CASES[name]
-    mol = gto.M(atom=geometry(geom), basis=basis)
+    cart = name in CART
+    mol = gto.M(atom=geometry(geom), basis=basis, cart=cart)
     auxmol = make_auxmol(mol)
+    if cart:
+        sys.path.insert(0, os.path.join(ROOT, 'tests'))
+        import cart_oracle as C
+        int2c2e, int3c2e_pairs = C.int2c2e, C.int3c2e_pairs
+    else:
+        int2c2e, int3c2e_pairs = O.int2c2e, O.int3c2e_pairs
     nao, naux = mol.nao, auxmol.nao
     loc = mol.ao_loc_nr()
     rng = np.random.RandomState(11)
     t0 = time.time()
     if omega is not None:
         mol._env[8] = omega
-    j2c = O.int2c2e(auxmol, omega=mol._env[8])
+    j2c = int2c2e(auxmol, omega=mol._env[8])
+    cond = 0.0
     try:
         low = scipy.linalg.cholesky(j2c, lower=True)
         chol = 1
         print(name, 'nao', nao, 'naux', naux, 'j2c + cholesky %.1f s' % (time.time() - t0), 'cond estimate %.2e'
               % (np.abs(np.diag(low)).max() / np.abs(np.diag(low)).min()) ** 2, flush=True)
+        if cart:
+            w = scipy.linalg.eigvalsh(j2c)
+            cond = float(w[-1] / w[0])
+            print('  metric condition number %.3e (eigenvalues %.3e .. %.3e)' % (cond, w[0], w[-1]), flush=True)
 
         def solve(x):
             return scipy.linalg.solve_triangular(low, x, lower=True, overwrite_b=True)
@@ -130,8 +172,8 @@ def main(name):
     small = name in SMALL
     pairs = pick_pairs(mol, rng, per_type=1 if small else 2)
     t0 = time.time()
-    j3c, col0 = O.int3c2e_pairs(mol, auxmol, pairs)
-    cd = solve(j3c)
+    j3c, col0 = int3c2e_pairs(mol, auxmol, pairs)
+    cd = solve(j3c.copy())
     cols, keep = [], []
     for p, (i, j) in enumerate(pairs):
         di, dj = loc[i + 1] - loc[i], loc[j + 1] - loc[j]
@@ -149,33 +191,33 @@ def main(name):
     sao = np.concatenate([np.arange(loc[s], loc[s + 1]) for s in S])
     t0 = time.time()
     slab_pairs = [(s, j) for s in S for j in range(mol.nbas)]
-    j3s, c0 = O.int3c2e_pairs(mol, auxmol, slab_pairs)
-    B = solve(j3s)     # [naux, sum_s d_s * nao]
-    del j3s
-    # reorder to B[P, s_ao, nu]
-    Bs = np.empty((naux, len(sao), nao))
-    row = 0
-    for si, s in enumerate(S):
-        ds = loc[s + 1] - loc[s]
-        for j in range(mol.nbas):
-            p = si * mol.nbas + j
-            dj = loc[j + 1] - loc[j]
-            Bs[:, row:row + ds, loc[j]:loc[j + 1]] = B[:, c0[p]:c0[p] + ds * dj].reshape(naux, ds, dj)
-        row += ds
-    del B
+    j3s, c0 = int3c2e_pairs(mol, auxmol, slab_pairs)
+    B = solve(j3s.copy())     # [naux, sum_s d_s * nao]
     print('  slab: shells', S, '->', len(sao), 'AOs, %.1f s' % (time.time() - t0), flush=True)
     t0 = time.time()
     c_s = slab_coeff(nao, nocc, sao)
     d_ss = 2.0 * c_s[sao].dot(c_s[sao].T)                      # occupation 2, as bench.py's SCF-like density
-    rho = np.einsum('psk,sk->p', Bs[:, :, sao], d_ss)
-    vj_rows = np.einsum('p,psn->sn', rho, Bs)                  # J[s, :] for s in sao
-    vk = np.zeros((nao, nao))
-    blk = 256
-    for p0 in range(0, naux, blk):
-        b = Bs[p0:p0 + blk]                                    # [pb, ns, nao]
-        t = np.matmul(d_ss, b)                                 # D_SS B_P[S,:]   [pb, ns, nao]
-        vk += b.reshape(-1, nao).T.dot(t.reshape(-1, nao))     # sum_{P,s} B[P,s,i] T[P,s,n]  (BLAS)
+    vj_rows, vk = slab_jk(B, S, c0, mol, loc, sao, d_ss)
     print('  J rows / K from the slab %.1f s; |K|max %.3g |J|max %.3g' % (time.time() - t0, abs(vk).max(), abs(vj_rows).max()), flush=True)
+    extra = {}
+    if cart:
+        # conditioning probe: the same J/K from integrals with NOISE relative noise (three draws), against the clean result
+        spread_j = spread_k = spread_c = 0.0
+        for seed in range(3):
+            nz = np.random.RandomState(100 + seed)
+            j2n = j2c * (1 + NOISE * nz.standard_normal(j2c.shape))
+            j2n = 0.5 * (j2n + j2n.T)
+            lown = scipy.linalg.cholesky(j2n, lower=True)
+            cdn = scipy.linalg.solve_triangular(lown, j3c * (1 + NOISE * nz.standard_normal(j3c.shape)), lower=True)[:, keep]
+            spread_c = max(spread_c, float(abs(cdn - cderi_cols).max()))
+            Bn = scipy.linalg.solve_triangular(lown, j3s * (1 + NOISE * nz.standard_normal(j3s.shape)), lower=True)
+            vjn, vkn = slab_jk(Bn, S, c0, mol, loc, sao, d_ss)
+            spread_j = max(spread_j, float(abs(vjn - vj_rows).max()))
+            spread_k = max(spread_k, float(abs(vkn - vk).max()))
+            print('  noise probe %d: max |dJ| %.2e  max |dK| %.2e  max |d cderi_cols| %.2e (running maxima)'
+                  % (seed, spread_j, spread_k, spread_c), flush=True)
+        extra = dict(cond=cond, noise=NOISE, noise_dj=spread_j, noise_dk=spread_k, noise_dcol=spread_c)
+    del j3s, B
     nsamp = 3000 if small else 6000
     ii, ll = rng.randint(nao, size=nsamp), rng.randint(nao, size=nsamp)
     ii[:len(sao)] = sao
@@ -184,7 +226,7 @@ def main(name):
     np.savez_compressed(out, nao=nao, naux=naux, nocc=nocc, omega=0.0 if omega is None else omega,
                         cols=cols, cderi_cols=cderi_cols, chol=chol, slab_shells=np.array(S), sao=sao, seed=7,
                         vj_rows=vj_rows, vk_idx=np.stack([ii, ll], 1), vk_val=vk[ii, ll], vk_fp=O.fp(vk), vk_absmax=abs(vk).max(),
-                        vk_diag=np.diag(vk).copy())
+                        vk_diag=np.diag(vk).copy(), **extra)
     print('  wrote', out, '%.1f MB' % (os.path.getsize(out) / 1e6), flush=True)
 
 
