@@ -202,6 +202,9 @@ typedef struct {
     double* c; double* rowmax; int8_t* qy; int32_t* ey;
 } b200jk_i8test;
 int b200jk_i8engine_test(b200jk_handle h, b200jk_i8test* t);
+/* Self-test of the Rys quadrature of the 4-center kernels: for every x[i] (>= 0, not NaN) the n-point rule (n = 1..9) that
+ * rys_root (jk_core.cuh) evaluates from the handle's device tables, in a kernel: u[count][n] roots, w[count][n] weights. */
+int b200jk_rys_test(b200jk_handle h, int n, int count, const double* x, double* u, double* w);
 int b200jk_get_stats(b200jk_handle h, b200jk_stats* out);
 const char* b200jk_last_error(b200jk_handle h);
 const char* b200jk_version(void);

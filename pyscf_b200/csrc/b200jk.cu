@@ -662,6 +662,50 @@ extern "C" int b200jk_fp64_peak(b200jk_handle h, double* tflops)
 #endif
 }
 
+namespace {
+// one x per thread: all n roots and weights, through the same rys_root the integral kernels call
+struct RysTestFn {
+    RysTables tb; int n; const double* x; double* u; double* w;
+    B2_HD void operator()(long i) const
+    {
+        for (int r = 0; r < n; r++) rys_root(tb, n, r, x[i], u[i * n + r], w[i * n + r]);
+    }
+};
+}  // namespace
+
+extern "C" int b200jk_rys_test(b200jk_handle h, int n, int count, const double* x, double* u, double* w)
+{
+    if (!h) return 1;
+    std::vector<void*> tmp;
+    int rc = 0;
+    try {
+        if (n < 1 || n > RYS_NMAX) throw std::runtime_error("b200jk_rys_test: n out of range 1..9");
+        if (count < 0 || (count > 0 && (!x || !u || !w))) throw std::runtime_error("b200jk_rys_test: bad arguments");
+        for (int i = 0; i < count; i++)
+            if (!(x[i] >= 0.0)) throw std::runtime_error("b200jk_rys_test: x must be >= 0 and not NaN");
+        if (count == 0) return 0;
+#ifndef B200JK_EMULATE
+        CK(cudaSetDevice(h->device));
+        stream_t st = h->stream;
+#else
+        stream_t st = 0;
+#endif
+        auto alloc = [&](size_t b) { void* p = dev_alloc(b); tmp.push_back(p); return p; };
+        double* dx = (double*)alloc((size_t)count * 8);
+        double* du = (double*)alloc((size_t)count * n * 8);
+        double* dw = (double*)alloc((size_t)count * n * 8);
+        h2d(dx, x, (size_t)count * 8, st);
+        launch_1d(count, RysTestFn{h->tb, n, dx, du, dw}, st);
+        d2h(u, du, (size_t)count * n * 8, st);
+        d2h(w, dw, (size_t)count * n * 8, st);
+#ifndef B200JK_EMULATE
+        CK(cudaStreamSynchronize(st));
+#endif
+    } catch (std::exception& e) { set_err(h, e.what()); rc = 2; }
+    for (void* p : tmp) dev_free(p);
+    return rc;
+}
+
 extern "C" int b200jk_get_stats(b200jk_handle h, b200jk_stats* out)
 {
     if (!h || !out) return 1;

@@ -45,7 +45,7 @@ SYMBOLS = ['b200jk_create', 'b200jk_create2', 'b200jk_destroy', 'b200jk_set_scre
            'b200jk_df_prepare_j', 'b200jk_df_direct_j', 'b200jk_df_stage_times', 'b200jk_df_set_cderi', 'b200jk_df_get_cderi_cols',
            'b200jk_incore_set_eri', 'b200jk_incore_jk', 'b200jk_set_class_costs',
            'b200jk_df_set_device_rows', 'b200jk_df_row_split', 'b200jk_df_stream_stats',
-           'b200jk_df_set_pair_tol', 'b200jk_df_pair_stats']
+           'b200jk_df_set_pair_tol', 'b200jk_df_pair_stats', 'b200jk_rys_test']
 
 
 def load(path=None):
@@ -83,6 +83,7 @@ def load(path=None):
     lib.b200jk_i8gemm_test.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_double_p, c_double_p, c_double_p,
                                        ctypes.c_int, ctypes.c_int]
     lib.b200jk_i8engine_test.argtypes = [vp, ctypes.POINTER(I8Test)]
+    lib.b200jk_rys_test.argtypes = [vp, ctypes.c_int, ctypes.c_int, c_double_p, c_double_p, c_double_p]
     lib.b200jk_df_set_kblock.argtypes = [vp, ctypes.c_int, ctypes.c_int]
     lib.b200jk_df_set_kmode.argtypes = [vp, ctypes.c_int, ctypes.c_int]
     lib.b200jk_df_set_device_rows.argtypes = [vp, ctypes.c_int]
