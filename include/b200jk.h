@@ -178,6 +178,13 @@ int b200jk_df_stream_stats(b200jk_handle h, int64_t* bytes, double* copy_ms, dou
  * pair_stats: ncol kept columns of the current tensor and npair = nao(nao+1)/2. */
 int b200jk_df_set_pair_tol(b200jk_handle h, double tol);
 int b200jk_df_pair_stats(b200jk_handle h, int64_t* ncol, int64_t* npair);
+/* Test hook: with on != 0 the next b200jk_df_build uses the identity as the metric transform (no factorisation, no
+ * eigen fallback): the tensor rows are the bare 3-center integrals (P|mu nu) in the reference layout, naux = number of
+ * auxiliary functions, and the assembled metric (P|Q) is kept for b200jk_df_get_metric_test.  Everything else of the build
+ * (auxiliary tables, 3-center batches, transforms, pair screening, host rows, sharding) runs unchanged.  Off by default;
+ * b200jk_df_direct_j refuses such a tensor. */
+int b200jk_df_set_raw_test(b200jk_handle h, int on);
+int b200jk_df_get_metric_test(b200jk_handle h, double* j2c, int naux);   /* [naux][naux], raw builds only */
 /* Self-test of the int8-slice tensor-core GEMM used by DF-K: C[M,N] = A[M,K] B[N,K]^T with `ns` 7-bit slices (split_rows +
  * gemm_ar_acc with automatic K ranges; upper triangle only when symmetric).  b200jk_i8engine_test with stage 2. */
 int b200jk_i8gemm_test(b200jk_handle h, int M, int N, int K, const double* A, const double* B, double* C, int ns,

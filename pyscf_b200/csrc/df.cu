@@ -80,6 +80,10 @@ struct DFState {
     double *d_fac = nullptr, *d_W = nullptr;
     double* d_Linv = nullptr;   // L^-1 row-major (integral-direct J: the metric solve as two streaming passes), made on first use
     bool fac_chol = true;
+    // raw test build (b200jk_df_set_raw_test): the rows are the bare (P|mu nu), there is no metric factor, and the assembled
+    // metric (P|Q) [naux_sph][naux_sph] is kept on the host for b200jk_df_get_metric_test
+    bool raw = false;
+    std::vector<double> raw_j2c;
     // J/K workspaces
     double *d_dmtril = nullptr, *d_rho = nullptr, *d_vjtril = nullptr, *d_A = nullptr, *d_Y = nullptr, *d_occ = nullptr,
            *d_dm = nullptr, *d_vk = nullptr, *d_vj = nullptr;
@@ -276,6 +280,10 @@ struct UnpackLongFn {   // G[l][P * ncolp + k] = A_P[l][k] (0 for the pad column
     }
 };
 struct IdentityFn { double* a; int n; B2_HD void operator()(long i) const { a[i * (long)n + i] = 1.0; } };
+struct IdentityRowsFn {   // rows [r0, r0 + nrow) of the n x n identity into a zero-filled a[nrow][n]
+    double* a; int n, r0;
+    B2_HD void operator()(long i) const { a[i * (long)n + r0 + i] = 1.0; }
+};
 struct GatherRowsFn {   // out[i][j] = X_colmajor[(r0+i), j]
     const double* x; double* out; int n, r0;
     B2_HD void operator()(long idx) const { long i = idx / n, j = idx - i * n; out[idx] = x[(r0 + i) + j * (long)n]; }
@@ -723,8 +731,19 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
         bool use_chol = true;
         std::vector<double> W;   // eig fallback: [naux_kept, naux] row-major
         int nkeep = nas;
+        // raw test build: keep (P|Q), skip the factorisation (the erf metric need not be positive definite) and use the identity
+        // as the metric transform below, so that the rows are the bare 3-center integrals
+        const bool raw = h->df_raw_test && !j_only;
+        if (raw) {
+            d->raw = true;
+            d->raw_j2c.resize((size_t)nas * nas);
+            d2h(d->raw_j2c.data(), d_j2c, (size_t)nas * nas * 8, st);
 #ifndef B200JK_EMULATE
-        {
+            CK(cudaStreamSynchronize(st));
+#endif
+        }
+#ifndef B200JK_EMULATE
+        if (!raw) {
             int lwork = 0;
             CKS(cusolverDnSetStream(d->cusolver, st));
             CKB(cublasSetStream(d->cublas, st));
@@ -771,7 +790,7 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
 #else
         std::vector<double> j2c_h((size_t)nas * nas);
         d2h(j2c_h.data(), d_j2c, (size_t)nas * nas * 8);
-        {
+        if (!raw) {
             std::vector<double> Lm = j2c_h;
             bool ok;
             cpu_cholesky_lower(Lm, nas, ok);
@@ -783,7 +802,8 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
 #endif
         d->naux = nkeep;
         d->fac_chol = use_chol;
-        d->d_fac = d_j2c;
+        if (raw) dev_free(d_j2c);
+        else d->d_fac = d_j2c;
         if (j_only) {   // integral-direct J only (b200jk_df_prepare_j): no tensor
 #ifndef B200JK_EMULATE
             CK(cudaStreamSynchronize(st));
@@ -799,8 +819,13 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
         const int nloc = r_hi - r_lo;
         d->build_rank = br; d->build_world = bw; d->row0 = r_lo; d->nrow = nloc;
         double* d_T = (double*)dev_alloc((size_t)std::max(nloc, 1) * nas * 8);
+        if (raw) {
+            dev_zero(d_T, (size_t)std::max(nloc, 1) * nas * 8, st);
+            IdentityRowsFn idr{d_T, nas, r_lo};
+            launch_1d(nloc, idr, st);
+        }
 #ifndef B200JK_EMULATE
-        if (use_chol) {
+        else if (use_chol) {
             // L^-1 by one triangular solve against the identity (naux^2, setup only), then gather this rank's rows
             double* d_inv = (double*)dev_alloc((size_t)nas * nas * 8);
             dev_zero(d_inv, (size_t)nas * nas * 8, st);
@@ -817,7 +842,7 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
             h2d(d_T, W.data() + (size_t)r_lo * nas, (size_t)nloc * nas * 8, st);
         }
 #else
-        {   // host: rows of L^-1 by forward substitution on unit vectors (tests only)
+        else {   // host: rows of L^-1 by forward substitution on unit vectors (tests only)
             std::vector<double> inv((size_t)nas * nas, 0.0);
             for (int c = 0; c < nas; c++) {
                 for (int i = c; i < nas; i++) {
@@ -963,6 +988,7 @@ extern "C" int b200jk_df_direct_j(b200jk_handle h, const double* dm, int n_dm, i
     if (!h) return 1;
     try {
         DFState* d = h->df;
+        if (d && d->raw) throw std::runtime_error("b200jk_df_direct_j: a raw test build (b200jk_df_set_raw_test) has no metric factor");
         if (!d || !d->d_fac) throw std::runtime_error("call b200jk_df_prepare_j (or b200jk_df_build) before b200jk_df_direct_j");
         if (nao != h->nsph) throw std::runtime_error("nao does not match the basis of this handle");
         if (n_dm < 1 || !dm || !vj) throw std::runtime_error("bad arguments");
@@ -1681,6 +1707,22 @@ extern "C" int b200jk_df_set_pair_tol(b200jk_handle h, double tol)
     if (!h) return 1;
     if (std::isnan(tol)) { set_err(h, "bad pair tolerance"); return 1; }
     h->df_pair_tol = tol > 0.0 ? tol : 0.0;
+    return 0;
+}
+
+extern "C" int b200jk_df_set_raw_test(b200jk_handle h, int on)
+{
+    if (!h) return 1;
+    h->df_raw_test = on != 0;
+    return 0;
+}
+
+extern "C" int b200jk_df_get_metric_test(b200jk_handle h, double* j2c, int naux)
+{
+    if (!h || !h->df || !j2c) { set_err(h, "call b200jk_df_build first"); return 1; }
+    if (!h->df->raw) { set_err(h, "the metric is kept by raw test builds only (b200jk_df_set_raw_test)"); return 1; }
+    if (naux != h->df->naux_sph) { set_err(h, "naux does not match the auxiliary basis of the tensor"); return 1; }
+    memcpy(j2c, h->df->raw_j2c.data(), (size_t)naux * naux * 8);
     return 0;
 }
 

@@ -192,6 +192,7 @@ struct b200jk_handle_s {
     void (*df_free)(DFState*) = nullptr;
     int df_dev_rows = -1;           // b200jk_df_set_device_rows: cap on the tensor rows kept in HBM (-1: automatic)
     double df_pair_tol = 0.0;       // b200jk_df_set_pair_tol: keep only the AO-pair columns with Schwarz bound >= tol (0: dense)
+    int df_raw_test = 0;            // b200jk_df_set_raw_test: build the bare 3-center integrals with the identity as metric transform
     double class_ms[NPC * NPC] = {0};
     double class_cost[NPC * NPC] = {0};   // measured class times handed in by the caller (b200jk_set_class_costs); 0 = use the model
     bool have_costs = false;
