@@ -212,6 +212,11 @@ int b200jk_i8engine_test(b200jk_handle h, b200jk_i8test* t);
 /* Self-test of the Rys quadrature of the 4-center kernels: for every x[i] (>= 0, not NaN) the n-point rule (n = 1..9) that
  * rys_root (jk_core.cuh) evaluates from the handle's device tables, in a kernel: u[count][n] roots, w[count][n] weights. */
 int b200jk_rys_test(b200jk_handle h, int n, int count, const double* x, double* u, double* w);
+/* Test hook of the on-device screening: the dm_cond table the last b200jk_direct_jk call screened with, dmc[nsh][nsh] over
+ * the device shells (one per shell and contraction column, sorted by angular momentum; nsh = n_dev_shells of the stats), and
+ * for each device shell its first AO in the caller's basis (ao_off[nsh], may be NULL): an index into the spherical AOs of
+ * a b200jk_create handle, into libcint's Cartesian AOs of a b200jk_create2(..., cart = 1) handle. */
+int b200jk_get_dm_cond_test(b200jk_handle h, double* dmc, int32_t* ao_off, int nsh);
 int b200jk_get_stats(b200jk_handle h, b200jk_stats* out);
 const char* b200jk_last_error(b200jk_handle h);
 const char* b200jk_version(void);

@@ -706,6 +706,23 @@ extern "C" int b200jk_rys_test(b200jk_handle h, int n, int count, const double* 
     return rc;
 }
 
+extern "C" int b200jk_get_dm_cond_test(b200jk_handle h, double* dmc, int32_t* ao_off, int nsh)
+{
+    if (!h) return 1;
+    try {
+        if (!dmc || nsh != h->nsh) throw std::runtime_error("b200jk_get_dm_cond_test: nsh must be the number of device shells");
+        if (!h->ws_ndm) throw std::runtime_error("b200jk_get_dm_cond_test: no b200jk_direct_jk call yet");
+#ifndef B200JK_EMULATE
+        CK(cudaSetDevice(h->device));
+#endif
+        d2h(dmc, h->d_dmc, (size_t)nsh * nsh * 8);
+        dev_sync();
+        if (ao_off)
+            for (int i = 0; i < nsh; i++) ao_off[i] = h->sh[i].sph_off;
+    } catch (std::exception& e) { set_err(h, e.what()); return 2; }
+    return 0;
+}
+
 extern "C" int b200jk_get_stats(b200jk_handle h, b200jk_stats* out)
 {
     if (!h || !out) return 1;

@@ -46,7 +46,7 @@ SYMBOLS = ['b200jk_create', 'b200jk_create2', 'b200jk_destroy', 'b200jk_set_scre
            'b200jk_incore_set_eri', 'b200jk_incore_jk', 'b200jk_set_class_costs',
            'b200jk_df_set_device_rows', 'b200jk_df_row_split', 'b200jk_df_stream_stats',
            'b200jk_df_set_pair_tol', 'b200jk_df_pair_stats', 'b200jk_rys_test', 'b200jk_df_set_raw_test',
-           'b200jk_df_get_metric_test']
+           'b200jk_df_get_metric_test', 'b200jk_get_dm_cond_test']
 
 
 def load(path=None):
@@ -98,6 +98,7 @@ def load(path=None):
     lib.b200jk_set_shard.argtypes = [vp, ctypes.c_int, ctypes.c_int]
     lib.b200jk_df_jk_device.argtypes = [vp, vp, ctypes.c_int, ctypes.c_int, vp, ctypes.c_int, ctypes.c_int, vp, vp]
     lib.b200jk_get_q_cond.argtypes = [vp, c_double_p, ctypes.c_int]
+    lib.b200jk_get_dm_cond_test.argtypes = [vp, c_double_p, c_int_p, ctypes.c_int]
     lib.b200jk_get_stats.argtypes = [vp, ctypes.POINTER(Stats)]
     lib.b200jk_set_stream.argtypes = [vp, vp]
     lib.b200jk_fp64_peak.argtypes = [vp, c_double_p]
