@@ -152,6 +152,12 @@ int b200jk_fp64_peak(b200jk_handle h, double* tflops);
  * ms[100]: entry [cb*10+ck], pair class id = l1*(l1+1)/2+l2 (ss,ps,pp,ds,dp,dd,fs,fp,fd,ff). */
 int b200jk_set_profile(b200jk_handle h, int on);
 int b200jk_get_class_times(b200jk_handle h, double* ms, int n);
+/* Launch shape of the 4-center class (cb ck), cb >= ck (pair class ids as above), as the direct build launches it on the handle's
+ * device; configures the kernel as a launch would.  info[n >= 9]: family (0 thread-per-quartet, 1 block), threads per CTA,
+ * dynamic shared memory per CTA (bytes), registers per thread, local memory per thread (bytes), CTAs per SM under the carve-out
+ * the library sets, that carve-out (percent, -1: none), CTAs per SM from registers and threads alone, 1 if bra and ket are
+ * swapped.  Fields a CPU build cannot know are -1. */
+int b200jk_class_launch_info(b200jk_handle h, int cb, int ck, int* info, int n);
 /* Caps on the blocking of the int8-slice K build (tests): at most max_block_rows auxiliary rows per K block and at most
  * max_resident_rows packed rows whose slices stay resident between calls (the rest are re-cut per block); -1 keeps the
  * automatic choice, which a cap can only shrink. */

@@ -586,6 +586,19 @@ extern "C" int b200jk_get_class_times(b200jk_handle h, double* ms, int n)
     return 0;
 }
 
+extern "C" int b200jk_class_launch_info(b200jk_handle h, int cb, int ck, int* info, int n)
+{
+    if (!h) return 1;
+    try {
+        if (!info || n < B2_LAUNCH_INFO_N || cb < 0 || cb >= NPC || ck < 0 || ck > cb) throw std::runtime_error("bad arguments");
+#ifndef B200JK_EMULATE
+        CK(cudaSetDevice(h->device));
+#endif
+        class_info(cb, ck, info);
+    } catch (std::exception& e) { set_err(h, e.what()); return 2; }
+    return 0;
+}
+
 // Measured per-class times (what b200jk_get_class_times returns after a profiled, unsharded build) as the cost table of the
 // multi-GPU partition.  Every rank must be given the SAME table (the host layer broadcasts rank 0's: pyscf_b200/parallel.py), since
 // the ranks derive the partition independently.  ms == NULL returns to the built-in model.

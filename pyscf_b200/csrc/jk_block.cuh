@@ -91,8 +91,7 @@ struct BlockSmem {
     SlotSmem<C> slot[GroupCfg<C>::NSLOT];
     BraInfo bra;
     PrimPair bprim[MAX_PRIM_PER_PAIR];                 // the stationary bra pair's primitive pairs (bulk async copy)
-    unsigned long long mbar_bra;                        // mbarriers of the bulk copies
-    unsigned long long mbar_slot[GroupCfg<C>::NSLOT];
+    unsigned long long mbar_bra;                        // mbarrier of that copy
     int klist[KCH_MAX];
     int nk;
     int next;
@@ -106,7 +105,6 @@ struct LaneCtx {
     int grp, lt, slot, valid;
     int ibp, ikp;
     int sr;          // omega < 0 only: 0 = Coulomb pass, 1 = (negated) erf pass of the current primitive quartet
-    unsigned kpar;   // phase parity of this slot's copy barrier
 };
 
 #if defined(__CUDA_ARCH__)
@@ -203,11 +201,6 @@ void group_proc(const KParams& P, BlockSmem<C>& sm, int grp, int nk, int bx,
                         if (P.same_class && kk == bx) f *= 0.5;
                         s.fac = f;
                         slot_set_cd<C>(s, kp.ABx, kp.ABy, kp.ABz);
-#if defined(__CUDA_ARCH__)
-                        bulk_g2s(s.kprim, P.prims + kp.prim_off, (unsigned)kp.nprim * (unsigned)sizeof(PrimPair), &sm.mbar_slot[L.slot]);
-#else
-                        for (int e2 = 0; e2 < kp.nprim; e2++) s.kprim[e2] = P.prims[kp.prim_off + e2];
-#endif
                     } else {
                         s.nprim_k = 0; s.nq = 0;
                     }
@@ -218,9 +211,6 @@ void group_proc(const KParams& P, BlockSmem<C>& sm, int grp, int nk, int bx,
             }
         B2_END
         group_sync<C>(grp);
-#if defined(__CUDA_ARCH__)
-        if (ctx.valid && sm.slot[ctx.slot].active) { bulk_wait(&sm.mbar_slot[ctx.slot], ctx.kpar); ctx.kpar ^= 1; }
-#endif
         constexpr bool sr_op = SR;   // erfc = Coulomb - erf: every primitive quartet is visited twice (omega < 0)
         if constexpr (C::PB > 1) {
             // ---- primitive batching: PB primitive quartets per round.  Quartet e of the slot (e < nq) is
@@ -246,7 +236,7 @@ void group_proc(const KParams& P, BlockSmem<C>& sm, int grp, int nk, int bx,
                                 const int sr = sr_op ? (e & 1) : 0;
                                 const int pq = sr_op ? (e >> 1) : e;
                                 const int ibp = pq / nkp, ikp = pq - ibp * nkp;
-                                phase_root_one<C>(s, b, r, sm.bprim[ibp], s.kprim[ikp], P.tb,
+                                phase_root_one<C>(s, b, r, sm.bprim[ibp], load_prim(P.prims + s.prim_off_k + ikp), P.tb,
                                                   sr_op ? (sr ? -P.omega : 0.0) : P.omega, (sr_op && sr) ? -1.0 : 1.0);
                             }
                         }
@@ -298,7 +288,7 @@ void group_proc(const KParams& P, BlockSmem<C>& sm, int grp, int nk, int bx,
                 if (L.valid) {
                     SlotSmem<C>& s = sm.slot[L.slot];
                     if (s.active && L.ibp < nbp)
-                        phase_roots<C>(s, L.t.g, sm.bprim[L.ibp], s.kprim[L.ikp], P.tb,
+                        phase_roots<C>(s, L.t.g, sm.bprim[L.ibp], load_prim(P.prims + s.prim_off_k + L.ikp), P.tb,
                                        sr_op ? (L.sr ? -P.omega : 0.0) : P.omega, (sr_op && L.sr) ? -1.0 : 1.0);
                 }
             B2_END
@@ -387,10 +377,6 @@ void jk_block(const KParams& P, int bx, int by, BlockSmem<C>& sm)
             sm.bra.same = bpair.same; sm.bra.idx = bx;
             sm.nk = 0; sm.next = 0;
 #if defined(__CUDA_ARCH__)
-            for (int i = 0; i < GC::NSLOT; i++) {
-                unsigned a = (unsigned)__cvta_generic_to_shared(&sm.mbar_slot[i]);
-                asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(a));
-            }
             {
                 unsigned a = (unsigned)__cvta_generic_to_shared(&sm.mbar_bra);
                 asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(a));
@@ -401,7 +387,6 @@ void jk_block(const KParams& P, int bx, int by, BlockSmem<C>& sm)
             for (int e2 = 0; e2 < bpair.nprim; e2++) sm.bprim[e2] = P.prims[bpair.prim_off + e2];
 #endif
         }
-        L.kpar = 0;
     B2_END
     B2_SYNC();
 #if defined(__CUDA_ARCH__)

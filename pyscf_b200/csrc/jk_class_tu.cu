@@ -8,7 +8,8 @@
 
 namespace b200jk {
 #define X(id, li, lj) \
-    void launch_bra_##id(int ck, const KParams& P, b2_stream_t st) { launch_ket<li, lj>(ck, P, st); }
+    void launch_bra_##id(int ck, const KParams& P, b2_stream_t st) { launch_ket<li, lj>(ck, P, st); } \
+    void info_bra_##id(int ck, int* out) { info_ket<li, lj>(ck, out); }
 #if !defined(B2_BRA_ID)
 B2_PAIR_CASES(X)
 #elif B2_BRA_ID == 0

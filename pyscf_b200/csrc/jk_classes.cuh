@@ -21,8 +21,8 @@ constexpr int lane_eff_permille(int g) { return g <= 32 ? (32 / g) * g * 1000 / 
 #define B2_PBMAX 1         // largest primitive batch (QClass::PB) of the block kernels; 1 = one primitive quartet per round
 #endif
 #ifndef B2_CARVEOUT
-#define B2_CARVEOUT 50     // shared-memory share of the 228 KB L1/shared array requested for the block kernels (percent)
-#endif
+#define B2_CARVEOUT -1     // shared-memory share (percent) of the L1/shared array requested for the block kernels; -1: per kernel,
+#endif                     // the smallest share that holds the CTAs its register budget allows (block_carveout)
 
 // number of bra-component parts per quartet: register block between 15 and 40 doubles (thread-local
 // horizontal recurrences are amortised over the block), then maximise lane use
@@ -155,21 +155,56 @@ typedef int b2_stream_t;
 #endif
 
 #ifndef B200JK_EMULATE
+inline void b2_check(cudaError_t e, const char* what)
+{
+    if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
+}
+
+// Shared-memory carve-out (percent of the SM's L1/shared array) of a block kernel: the smallest one that holds as many CTAs as its
+// registers and threads allow, so that the rest of the array stays L1 for what the kernels read through it (Rys table rows,
+// primitive pairs, density).  The CUDA driver rounds the percentage up to the next capacity the SM supports.
+inline int block_carveout(const void* kern, int nt, size_t smem)
+{
+    int dev = 0, smem_sm = 0, reserved = 0, ctas = 0;
+    b2_check(cudaGetDevice(&dev), "cudaGetDevice");
+    b2_check(cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev), "cudaDeviceGetAttribute");
+    b2_check(cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev), "cudaDeviceGetAttribute");
+    b2_check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, kern, nt, 0), "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
+    const long per_cta = (long)smem + reserved;
+    if (ctas * per_cta > smem_sm) ctas = (int)(smem_sm / per_cta);
+    if (ctas < 1) ctas = 1;
+    const long pct = (100 * ctas * per_cta + smem_sm - 1) / smem_sm;
+    return pct < 100 ? (int)pct : 100;
+}
+
+// The entry point a block class launches (only that one is instantiated), configured on first use: dynamic shared memory and
+// carve-out.  carveout: the percentage set.
+typedef void (*block_kernel_t)(const KParams);
+template <class C, bool SR>
+block_kernel_t block_kernel(int& carveout)
+{
+    block_kernel_t kern = nullptr;
+    if constexpr (GroupCfg<C>::NT <= 192 && class_caps_registers(C::LI, C::LJ, C::LK, C::LL)) kern = jk_class_kernel_2cta<C, SR>;
+    else kern = jk_class_kernel<C, SR>;
+    static int carve = -1;
+    if (carve < 0) {
+        const size_t smem = sizeof(BlockSmem<C>);
+        b2_check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute");
+        static const int carve_env = getenv("B200JK_CARVEOUT") ? atoi(getenv("B200JK_CARVEOUT")) : -1;   // tuning experiment
+        int c = carve_env >= 0 ? carve_env : B2_CARVEOUT;
+        if (c < 0) c = block_carveout((const void*)kern, GroupCfg<C>::NT, smem);
+        b2_check(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, c), "cudaFuncSetAttribute");
+        carve = c;
+    }
+    carveout = carve;
+    return kern;
+}
+
 template <class C, bool SR>
 void launch_block_kernel(const KParams& P, dim3 grid, int nt, size_t smem, b2_stream_t st)
 {
-    void (*kern)(const KParams) = nullptr;      // only the chosen entry point is instantiated
-    if constexpr (GroupCfg<C>::NT <= 192 && class_caps_registers(C::LI, C::LJ, C::LK, C::LL)) kern = jk_class_kernel_2cta<C, SR>;
-    else kern = jk_class_kernel<C, SR>;
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) throw std::runtime_error(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e));
-        // leave half of the 228 KB for L1 (Rys tables, density blocks); the other half lets several CTAs co-reside
-        static const int carve_env = getenv("B200JK_CARVEOUT") ? atoi(getenv("B200JK_CARVEOUT")) : -1;   // tuning experiment
-        cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, carve_env >= 0 ? carve_env : B2_CARVEOUT);
-        configured = true;
-    }
+    int carveout = 0;
+    block_kernel_t kern = block_kernel<C, SR>(carveout);
     kern<<<grid, nt, smem, st>>>(P);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) throw std::runtime_error(std::string("jk_class_kernel launch: ") + cudaGetErrorString(e));
@@ -227,6 +262,45 @@ void launch_one(KParams P, b2_stream_t st)
 #endif
 }
 
+// Launch shape of a class as launch_one launches it (the omega >= 0 entry point), out[B2_LAUNCH_INFO_N]:
+//   [0] family: 0 thread-per-quartet, 1 block     [1] threads per CTA     [2] dynamic shared memory per CTA (bytes)
+//   [3] registers per thread     [4] local memory per thread (bytes; > 0 means spills)
+//   [5] CTAs per SM by the occupancy API under the carve-out set     [6] carve-out set (percent; -1: none)
+//   [7] CTAs per SM that registers and threads alone allow     [8] 1 if launched with bra and ket swapped (use_swapped)
+// The CPU emulation fills [0]-[2] and [8] only (-1 elsewhere).
+constexpr int B2_LAUNCH_INFO_N = 9;
+template <int LI, int LJ, int LK, int LL>
+void info_one(int* out)
+{
+    using Cfg = ClassCfg<LI, LJ, LK, LL>;
+    using C = typename Cfg::C;
+    for (int i = 0; i < B2_LAUNCH_INFO_N; i++) out[i] = -1;
+    const void* kern = nullptr;
+    size_t smem = 0;
+    if constexpr (TpqCfg<C>::eligible) {
+        out[0] = 0; out[1] = TpqCfg<C>::NT;
+#ifndef B200JK_EMULATE
+        kern = (const void*)jk_tpq_kernel<C, false>;
+#endif
+    } else {
+        out[0] = 1; out[1] = Cfg::NT; smem = sizeof(BlockSmem<C>);
+#ifndef B200JK_EMULATE
+        kern = (const void*)block_kernel<C, false>(out[6]);
+#endif
+    }
+    out[2] = (int)smem;
+#ifndef B200JK_EMULATE
+    cudaFuncAttributes fa;
+    b2_check(cudaFuncGetAttributes(&fa, kern), "cudaFuncGetAttributes");
+    out[3] = fa.numRegs;
+    out[4] = (int)fa.localSizeBytes;
+    b2_check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&out[5], kern, out[1], smem), "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
+    b2_check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&out[7], kern, out[1], 0), "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
+#else
+    (void)kern;
+#endif
+}
+
 // pair class id = l1*(l1+1)/2 + l2  (l1 >= l2)
 #define B2_PAIR_CASES(X) \
     X(0, 0, 0) X(1, 1, 0) X(2, 1, 1) X(3, 2, 0) X(4, 2, 1) X(5, 2, 2) X(6, 3, 0) X(7, 3, 1) X(8, 3, 2) X(9, 3, 3)
@@ -262,10 +336,42 @@ void launch_ket(int ck, const KParams& P, b2_stream_t st)
     throw std::runtime_error("bad ket class");
 }
 
+template <int LI, int LJ>
+void info_ket(int ck, int* out)
+{
+    constexpr int cb = LI * (LI + 1) / 2 + LJ;
+    switch (ck) {
+#define X(id, lk, ll)                                                      \
+    case id:                                                               \
+        if constexpr (id <= cb || use_swapped(id, cb)) info_one<LI, LJ, lk, ll>(out); \
+        return;
+        B2_PAIR_CASES(X)
+#undef X
+    }
+    throw std::runtime_error("bad ket class");
+}
+
 // one translation unit per bra pair class (jk_class_tu.cu compiled with -DB2_BRA_ID=<id>)
-#define X(id, li, lj) void launch_bra_##id(int ck, const KParams& P, b2_stream_t st);
+#define X(id, li, lj) void launch_bra_##id(int ck, const KParams& P, b2_stream_t st); void info_bra_##id(int ck, int* out);
 B2_PAIR_CASES(X)
 #undef X
+
+// launch shape of the class (cb ck), cb >= ck, as launch_class launches it (see info_one)
+inline void class_info(int cb, int ck, int* out)
+{
+    const bool swapped = cb > ck && use_swapped(cb, ck);
+    if (swapped) { int t = cb; cb = ck; ck = t; }
+    switch (cb) {
+#define X(id, li, lj)                  \
+    case id:                           \
+        info_bra_##id(ck, out);        \
+        out[8] = swapped ? 1 : 0;      \
+        return;
+        B2_PAIR_CASES(X)
+#undef X
+    }
+    throw std::runtime_error("bad bra class");
+}
 
 inline void launch_class(int cb, int ck, const KParams& P0, b2_stream_t st)
 {

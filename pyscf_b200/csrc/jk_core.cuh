@@ -188,8 +188,9 @@ struct alignas(16) SlotSmem {
     // 2-D integrals after the vertical recurrence AND the ket transfer (k -> l), ready for per-thread bra transfer:
     // H[dir][root][(l*(LK+1)+k)*NB1P + n]; z carries weight*prefactor.  Rows of n are contiguous (LDS.128).
     // The leading index is the primitive quartet of the current batch (C::PB of them, see QClass).
+    // The ket's primitive pairs are not staged here: phase A reads the one it needs from global memory (load_prim), so a
+    // slot costs shared memory only for what phases B and D share between lanes.
     double H[C::PB][3][C::NR][C::HSP];
-    PrimPair kprim[MAX_PRIM_PER_PAIR];   // this ket's primitive pairs, staged by one bulk async copy (TMA, UBLKCP) per batch
     double U[C::PB][C::NR], W[C::PB][C::NR];
     double pc[C::PB][14];        // p, q, PA[3], QC[3], PQ[3], 1/(p+q), 0.5/p, 0.5/q
     double ccd[3][C::LL + 1][C::LL + 1];  // binom(l,t) CD^(l-t)
