@@ -25,6 +25,9 @@
  *   b200jk_df_direct_j       -> CVHFnr3c2e_* passes over int3c2e  pyscf/lib/vhf/optimizer.c:305-370
  *   b200jk_df_jk             df_jk.get_jk                        pyscf/df/df_jk.py:280-413
  *                            -> AO2MOnr_e2_drv + NPdgemm         pyscf/lib/ao2mo/nr_ao2mo.c:1240, np_helper/npdot.c:32
+ *   b200jk_df_ao2mo          DF.ao2mo = get_mo_eri               pyscf/df/df.py:278-296
+ *                            -> _ao2mo.nr_e2 + lib.dot           pyscf/ao2mo/_ao2mo.py:157, pyscf/lib/ao2mo/nr_ao2mo.c:1240
+ *   b200jk_df_get_ao_eri     DF.get_eri = get_ao_eri             pyscf/df/df.py:269-276 (+ ao2mo.restore(8))
  *   b200jk_get_stats         (no reference equivalent; logger.timer 'vj and vk' pyscf/scf/hf.py:2158)
  *
  * Conventions: all matrices are C-contiguous fp64 in the reference's spherical AO order;
@@ -128,6 +131,25 @@ int b200jk_df_get_cderi(b200jk_handle h, double* out, int r0, int nr);
 /* Columns cols[ncols] (packed AO-pair indices mu(mu+1)/2+nu, mu >= nu) of all LOCAL rows: out[nrow_local][ncols] — numpy
  * slicing dfobj._cderi[:, cols] on the reference's ndarray tensor (pyscf/df/df.py:116); samples a tensor too large to copy. */
 int b200jk_df_get_cderi_cols(b200jk_handle h, double* out, const int64_t* cols, int ncols);
+
+/* MO integrals from the tensor: DF.ao2mo = get_mo_eri (pyscf/df/df.py:278-296: _ao2mo.nr_e2 on each row block + lib.dot).
+ * c1..c4: host [nao][n1..n4] C-contiguous coefficients over the handle's AOs (Cartesian ones on a Cartesian handle).
+ * out[nij][nkl] (host) = sum_P L[P, ij] L'[P, kl], L[P, ij] = sum_{mu nu} c1[mu,i] B_P[mu,nu] c2[nu,j].  s2_12 != 0 (c1 and c2 the
+ * same set, n1 == n2): ij = i(i+1)/2 + j, i >= j, nij = n1(n1+1)/2; else ij = i n2 + j.  Pair (3,4) alike; c3 == NULL: pair (3,4)
+ * is pair (1,2) (the reference's sym, df.py:286-294) and only the lower output tiles are computed where a band allows it.
+ * Stage 1 (half transforms, all local rows kept on the device) and stage 2 (output bands through pinned staging) run on FP64
+ * tensor-core GEMMs (df_ao2mo.cuh); pair-screened tensors and host rows are read as b200jk_df_jk reads them.  Fails with a
+ * message when L (and L') do not fit in device memory; a sharded tensor is refused. */
+int b200jk_df_ao2mo(b200jk_handle h, const double* c1, int n1, const double* c2, int n2, int s2_12, const double* c3, int n3,
+                    const double* c4, int n4, int s2_34, double* out);
+/* AO integrals from the tensor: DF.get_eri = get_ao_eri (pyscf/df/df.py:269-276): ao2mo.restore(8, B^T B, nao), the lower
+ * triangle row by row of the [npair, npair] matrix sum_P B[P,:]^T B[P,:] (npair = nao(nao+1)/2): out_s8[npair(npair+1)/2]. */
+int b200jk_df_get_ao_eri(b200jk_handle h, double* out_s8);
+/* Test hook: at most max_rows output rows per band of b200jk_df_ao2mo / b200jk_df_get_ao_eri (-1: automatic, <= 256 MiB). */
+int b200jk_df_set_ao2mo_tile(b200jk_handle h, int max_rows);
+/* Times of the last b200jk_df_ao2mo / b200jk_df_get_ao_eri (no reference equivalent): ms[0] stage-1 and ms[1] stage-2 device
+ * time (CUDA events around the launches), ms[2] host wall time of the whole call including the copies; n <= 3 entries. */
+int b200jk_df_ao2mo_times(b200jk_handle h, double* ms, int n);
 
 /* Schwarz table q_cond[nbas,nbas] in the reference's (contracted, spherical-order) shell indexing. */
 int b200jk_get_q_cond(b200jk_handle h, double* q_cond, int nbas);

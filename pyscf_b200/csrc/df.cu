@@ -4,6 +4,8 @@
 //                     (P|Q), (ij|P) from the Rys kernels in df_block.cuh, Cholesky/TRSM on device
 //                     (eigendecomposition fallback with `lindep`, incore.py:150-158,263-270)
 //   b200jk_df_jk    : J = cderi^T (cderi . dmtril) ; K = sum_P (P|.i)(P|.i)^T  <- df_jk.get_jk, pyscf/df/df_jk.py:280-413
+//   b200jk_df_ao2mo, b200jk_df_get_ao_eri : MO / AO integrals from the tensor      <- DF.ao2mo / get_eri, pyscf/df/df.py:269-296
+//                     (df_ao2mo.cuh, FP64 tensor-core GEMMs)
 // The tensor stays resident in HBM in the reference's own layout (row P, packed lower triangle mu>=nu).
 #include "host_common.hpp"
 #include "df_classes.cuh"
@@ -112,6 +114,10 @@ struct DFState {
     cudaEvent_t ev_free[2] = {nullptr, nullptr};
 #endif
     double stage_ms[B200JK_DF_NSTAGE] = {0}; int stage_n[B200JK_DF_NSTAGE] = {0};
+    // MO transforms (df_ao2mo.cuh): device ms of stage 1 and stage 2 and host ms of the last call; test cap on the output band rows
+    double ao2mo_ms[3] = {0, 0, 0};
+    int ao2mo_tile_rows = -1;
+    double* h_pin[2] = {nullptr, nullptr}; size_t pin_cap = 0;   // pinned staging of the output bands, kept between calls
 };
 
 namespace {
@@ -125,6 +131,7 @@ void df_free(DFState* d)
     for (cudaEvent_t e : d->ev_free) if (e) cudaEventDestroy(e);
     if (d->cp_stream) cudaStreamDestroy(d->cp_stream);
     if (d->h_cderi) cudaFreeHost(d->h_cderi);
+    for (double* p : d->h_pin) if (p) cudaFreeHost(p);
 #else
     free(d->h_cderi);
 #endif
@@ -1755,3 +1762,5 @@ extern "C" int b200jk_df_set_kmode(b200jk_handle h, int mode, int nslices)
     h->df->k_mode = mode; h->df->k_slices = nslices;
     return 0;
 }
+
+#include "df_ao2mo.cuh"

@@ -2,7 +2,8 @@
 
 Mirrors (names, argument meaning, shapes):
   * df.DF(mol, auxbasis): build(), reset(), get_naoaux(), loop(), get_jk(dm, hermi, with_j, with_k,
-    direct_scf_tol, omega), range_coulomb(omega)                      pyscf/df/df.py:56-333
+    direct_scf_tol, omega), range_coulomb(omega), ao2mo = get_mo_eri, get_eri = get_ao_eri
+                                                                       pyscf/df/df.py:56-333
   * df_jk.get_jk algebra incl. the mo_coeff/mo_occ fast path           pyscf/df/df_jk.py:280-413
   * addons.make_auxmol / predefined auxiliary basis                    pyscf/df/addons.py:230-361
   * density_fit(mf) installer                                          pyscf/df/df_jk.py:31-107
@@ -38,6 +39,15 @@ def _check_aux_cart(mol, auxmol):
         raise NotImplementedError('Interface for int3c2e_ssc')
     if _is_cart(mol) and not _is_cart(auxmol):
         raise RuntimeError('Cartesian orbitals for mol and spherical orbitals for auxmol not supported')
+
+
+def _iden_coeffs(mo1, mo2):
+    """ao2mo.incore.iden_coeffs (pyscf/ao2mo/incore.py:239-241): the same object, or equal shapes within 1e-13 (empty sets of
+    equal shape count as equal)."""
+    if mo1 is mo2:
+        return True
+    a, b = np.asarray(mo1), np.asarray(mo2)
+    return a.shape == b.shape and bool(a.size == 0 or abs(a - b).max() < 1e-13)
 
 
 class DF:
@@ -350,6 +360,72 @@ class DF:
                 h.check(h.lib.b200jk_df_jk(h._h, _lib.dptr(dms[k:k + 1]), 1, nao, _lib.dptr(orbo[k][None]), nocc, int(hermi), None,
                                            _lib.dptr(vk[k:k + 1])), 'b200jk_df_jk')
         return (None if vj is None else vj.reshape(shape)), (None if vk is None else vk.reshape(shape))
+
+    # ---- MO / AO integrals from the tensor ------------------------------------------------------------
+    def ao2mo(self, mo_coeffs, compact=True):
+        """(ij|kl) = sum_P L[P, ij] L[P, kl], L[P, ij] = C1[:, i]^T B_P C2[:, j], on the GPU: DF.ao2mo (pyscf/df/df.py:278-296),
+        what mp.MP2, DF-CASSCF and DF-NEVPT2 call on mf.with_df.
+
+        mo_coeffs: one [nao, n] array (four equal sets) or a sequence of four.  Pair (1,2) is packed s2 (row i(i+1)/2 + j,
+        i >= j) when `compact` and its two sets are identical in the sense of iden_coeffs (pyscf/ao2mo/incore.py:239-241),
+        else s1 (row i n2 + j); pair (3,4) alike.  Returns [nij, nkl] float64."""
+        if self.shard is not None:
+            raise NotImplementedError('DF.ao2mo on a sharded tensor (DF(shard=...)) is not implemented')
+        if isinstance(mo_coeffs, np.ndarray) and mo_coeffs.ndim == 2:
+            mo_coeffs = (mo_coeffs,) * 4
+        if len(mo_coeffs) != 4:
+            raise ValueError('DF.ao2mo needs one [nao, n] array or four of them, got %d' % len(mo_coeffs))
+        self.get_naoaux()
+        nao = self.nao
+        cs = []
+        for c in mo_coeffs:
+            a = np.asarray(c)
+            if np.iscomplexobj(a):
+                raise NotImplementedError('DF.ao2mo: complex MO coefficients are not supported')
+            if a.ndim != 2 or a.shape[0] != nao:
+                raise ValueError('DF.ao2mo: MO coefficients must be [nao, n] with nao = %d, got shape %s' % (nao, a.shape))
+            cs.append(a)
+        # _conc_mos (pyscf/ao2mo/incore.py:244-262): s2 only for identical double-precision sets
+        s12 = bool(compact) and np.result_type(cs[0], cs[1]) == np.double and _iden_coeffs(mo_coeffs[0], mo_coeffs[1])
+        s34 = bool(compact) and np.result_type(cs[2], cs[3]) == np.double and _iden_coeffs(mo_coeffs[2], mo_coeffs[3])
+        sym = s12 == s34 and _iden_coeffs(mo_coeffs[0], mo_coeffs[2]) and _iden_coeffs(mo_coeffs[1], mo_coeffs[3])
+        n = [a.shape[1] for a in cs]
+        nij = n[0] * (n[0] + 1) // 2 if s12 else n[0] * n[1]
+        nkl = n[2] * (n[2] + 1) // 2 if s34 else n[2] * n[3]
+        out = np.empty((nij, nkl))
+        if out.size == 0:
+            return out
+        cs = [np.ascontiguousarray(a, dtype=np.float64) for a in cs]
+        h = self._handle
+        if sym:
+            h.check(h.lib.b200jk_df_ao2mo(h._h, _lib.dptr(cs[0]), n[0], _lib.dptr(cs[1]), n[1], int(s12), None, 0, None, 0, 0,
+                                          _lib.dptr(out)), 'b200jk_df_ao2mo')
+        else:
+            h.check(h.lib.b200jk_df_ao2mo(h._h, _lib.dptr(cs[0]), n[0], _lib.dptr(cs[1]), n[1], int(s12), _lib.dptr(cs[2]), n[2],
+                                          _lib.dptr(cs[3]), n[3], int(s34), _lib.dptr(out)), 'b200jk_df_ao2mo')
+        return out
+    get_mo_eri = ao2mo
+
+    def get_eri(self):
+        """ao2mo.restore(8, sum_P B[P]^T B[P], nao) on the GPU (DF.get_eri, pyscf/df/df.py:269-276): the lower triangle, row by
+        row, of the [npair, npair] AO-pair matrix (npair = nao(nao+1)/2), a vector of npair(npair+1)/2."""
+        if self.shard is not None:
+            raise NotImplementedError('DF.get_eri on a sharded tensor (DF(shard=...)) is not implemented')
+        self.get_naoaux()
+        npair = self.nao * (self.nao + 1) // 2
+        out = np.empty(npair * (npair + 1) // 2)
+        h = self._handle
+        h.check(h.lib.b200jk_df_get_ao_eri(h._h, _lib.dptr(out)), 'b200jk_df_get_ao_eri')
+        return out
+    get_ao_eri = get_eri
+
+    def ao2mo_times(self):
+        """Milliseconds of the last ao2mo / get_eri: {'stage1', 'stage2'} device time of the half transforms and of the
+        output GEMMs (CUDA events), 'total' host time of the whole call including the copies to the caller."""
+        h = self._handle
+        ms = np.zeros(3)
+        h.check(h.lib.b200jk_df_ao2mo_times(h._h, _lib.dptr(ms), 3), 'b200jk_df_ao2mo_times')
+        return {'stage1': float(ms[0]), 'stage2': float(ms[1]), 'total': float(ms[2])}
 
     def stats(self):
         return self._handle.stats()
