@@ -38,6 +38,229 @@
 
 using namespace b200jk;
 
+// ---- device / host row split ---------------------------------------------------------------------
+// bytes of int8 slices per packed row, and what the K build needs besides the tensor: the per-block slice stack and 12 GB of
+// workspaces (the reserve the slice-residency decision keeps)
+static size_t slice_row_bytes(int nao, int ns) { return (size_t)ns * nao * (((size_t)nao + 127) / 128 * 128); }
+static size_t k_reserve_bytes(int nao, int kb, int ns) { return (size_t)(kb + 1) * slice_row_bytes(nao, ns) + (12UL << 30); }
+// rows per K block of a rank holding nloc rows: the block unpacked to nao x nao takes at most 2 GiB
+static int k_block_rows(int nao, int nloc)
+{
+    return (int)std::max<long>(1, std::min<long>(std::max(nloc, 1), (2048L << 20) / ((long)nao * nao * 8)));
+}
+// rows [lo, hi) of n that rank `rank` of `world` owns
+static void shard_range(long n, int rank, int world, int& lo, int& hi)
+{
+    lo = (int)(n * rank / world); hi = (int)(n * (rank + 1) / world);
+}
+
+// MemAvailable of /proc/meminfo in bytes (0 when it cannot be read)
+static size_t host_mem_available()
+{
+    FILE* f = fopen("/proc/meminfo", "r");
+    if (!f) return 0;
+    char line[256];
+    size_t kb = 0;
+    while (fgets(line, sizeof line, f))
+        if (sscanf(line, "MemAvailable: %zu kB", &kb) == 1) break;
+    fclose(f);
+    return kb * 1024;
+}
+
+// Where the local rows of the tensor live: rows [0, n_dev) in HBM (DFState::d_cderi), rows [n_dev, nrow) in pinned host memory.
+// The host rows are streamed through the two device staging buffers d_stage (stage_rows rows each) once per J/K or MO transform
+// call.  n_dev == nrow when the tensor fits next to the K workspaces.
+struct RowSplit {
+    int n_dev = 0, stage_rows = 0;
+    long ld = 0;                       // row length in doubles
+    double* h_cderi = nullptr;
+    double* d_stage[2] = {nullptr, nullptr};
+    int64_t bytes = 0; double copy_ms = 0.0, exposed_ms = 0.0;   // last timed walk (b200jk_df_stream_stats)
+    int timed_blocks = 0;
+#ifndef B200JK_EMULATE
+    // H2D copies run on cp_stream; per staged block, events at copy start / end and around the wait of the compute stream
+    // (exposed copy time); ev_free[slot] marks the compute on a staging buffer done
+    cudaStream_t cp_stream = nullptr;
+    cudaEvent_t ev_start = nullptr, ev_free[2] = {nullptr, nullptr};
+    std::vector<cudaEvent_t> blk_ev;
+#endif
+
+    ~RowSplit()
+    {
+#ifndef B200JK_EMULATE
+        for (cudaEvent_t e : blk_ev) cudaEventDestroy(e);
+        for (cudaEvent_t e : {ev_start, ev_free[0], ev_free[1]}) if (e) cudaEventDestroy(e);
+        if (cp_stream) cudaStreamDestroy(cp_stream);
+        if (h_cderi) cudaFreeHost(h_cderi);
+#else
+        free(h_cderi);
+#endif
+        dev_free(d_stage[0]); dev_free(d_stage[1]);
+    }
+
+    // Decide how many of this rank's nloc rows of ld_ doubles stay in HBM and allocate them in *dev (zero-filled on request), the
+    // pinned host rows and the two staging buffers.  With the automatic split (h->df_dev_rows = -1) every row stays on the device
+    // when the tensor fits next to the K reserve; otherwise the device keeps as many rows as leave room for that reserve and the
+    // staging buffers.  The host part is checked against MemAvailable before it is allocated.  Returns an empty string on
+    // success, else the error (the caller frees the state).
+    std::string plan(b200jk_handle h, int nloc, long ld_, int k_slices, bool zero_fill, double** dev, stream_t st)
+    {
+        const int nao = h->nsph;
+        ld = ld_;
+        const size_t rowb = (size_t)ld * 8;
+        const size_t stage_cap = std::max<size_t>(1, std::min<size_t>(std::max(nloc, 1), (1UL << 30) / rowb));   // rows in 1 GiB
+        long nd = nloc;
+        if (h->df_dev_rows >= 0) nd = std::min<long>(nloc, h->df_dev_rows);
+#ifndef B200JK_EMULATE
+        else {
+            size_t freeb = 0, totb = 0;
+            CK(cudaMemGetInfo(&freeb, &totb));
+            const double reserve = (double)k_reserve_bytes(nao, k_block_rows(nao, nloc), k_slices);
+            if ((double)nloc * rowb + reserve > (double)freeb) {
+                const double avail = (double)freeb - reserve - 2.0 * stage_cap * rowb - (double)(1UL << 30);
+                nd = avail > 0 ? std::min<long>(nloc, (long)(avail / rowb)) : 0;
+            }
+        }
+#endif
+        const long n_host = nloc - nd;
+        if (n_host > 0) {
+            const size_t hbytes = (size_t)n_host * rowb, avail = host_mem_available();
+            if (avail && (double)hbytes > 0.9 * (double)avail - (double)(2UL << 30)) {
+                char buf[320];
+                snprintf(buf, sizeof buf, "the DF tensor does not fit: %ld of its %d rows (%.1f GB) exceed the device and need pinned "
+                         "host memory, but MemAvailable is %.1f GB", n_host, nloc, hbytes / 1e9, avail / 1e9);
+                return buf;
+            }
+        }
+        n_dev = (int)nd;
+        *dev = (double*)dev_alloc((size_t)std::max<long>(nd, 1) * rowb);
+        if (zero_fill) dev_zero(*dev, (size_t)std::max<long>(nd, 1) * rowb, st);
+        if (n_host > 0) {
+            stage_rows = (int)std::min<long>((long)stage_cap, n_host);
+#ifndef B200JK_EMULATE
+            CK(cudaHostAlloc((void**)&h_cderi, (size_t)n_host * rowb, cudaHostAllocDefault));
+#else
+            h_cderi = (double*)malloc((size_t)n_host * rowb);
+            if (!h_cderi) throw std::runtime_error("host rows of the DF tensor: out of memory");
+#endif
+            for (double*& s : d_stage) s = (double*)dev_alloc((size_t)stage_rows * rowb);
+        }
+        return "";
+    }
+
+    double* host_row(long r) const { return h_cderi + (size_t)(r - n_dev) * ld; }
+    // end of the device rows of the local range [r_lo, r_hi): rows [r_lo, dev_end) are in HBM, the rest are streamed
+    int dev_end(int r_lo, int r_hi) const { return std::max(r_lo, std::min(r_hi, n_dev)); }
+
+    // local rows [r0, r0 + nr) into dst[nr][ld] on the host
+    void read(double* dst, const double* dev, int r0, int nr) const
+    {
+        const int nd = std::max(0, std::min(r0 + nr, n_dev) - r0);
+        if (nd > 0) {
+            d2h(dst, dev + (size_t)r0 * ld, (size_t)nd * ld * 8);
+            dev_sync();
+        }
+        if (nr > nd) memcpy(dst + (size_t)nd * ld, host_row(r0 + nd), (size_t)(nr - nd) * ld * 8);
+    }
+
+#ifndef B200JK_EMULATE
+    cudaStream_t copy_stream()     // made on first use, with its events
+    {
+        if (!cp_stream) {
+            CK(cudaStreamCreateWithFlags(&cp_stream, cudaStreamNonBlocking));
+            for (cudaEvent_t* e : {&ev_start, &ev_free[0], &ev_free[1]}) CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+        }
+        return cp_stream;
+    }
+#endif
+
+    // Visit the local rows [r_lo, r_hi) on the compute stream st: visit(src, r0, nr) once for the rows in HBM, in place (also
+    // when the range has no rows at all), then once per block of up to hb host rows staged in d_stage[b & 1].  Blocks 0 and 1 are
+    // copied while the device rows are visited, block b + 2 once st is done with block b; the copies follow the work queued on st
+    // before the walk.  timed: record the copy and wait events of every block and count the bytes (read_times gives the times).
+    template <class F>
+    void walk(const double* dev, int r_lo, int r_hi, int hb, bool timed, stream_t st, F visit)
+    {
+        const int r_dev = dev_end(r_lo, r_hi);
+        const int nblk = r_dev < r_hi ? (r_hi - r_dev + hb - 1) / hb : 0;
+        if (timed) { bytes = 0; copy_ms = 0.0; exposed_ms = 0.0; timed_blocks = nblk; }
+#ifndef B200JK_EMULATE
+        if (nblk > 0) {
+            copy_stream();
+            while (blk_ev.size() < 4 * (size_t)nblk) { cudaEvent_t e; CK(cudaEventCreate(&e)); blk_ev.push_back(e); }
+            CK(cudaEventRecord(ev_start, st));
+            CK(cudaStreamWaitEvent(cp_stream, ev_start, 0));
+        }
+#endif
+        auto copy = [&](int b) {
+            const int a = r_dev + b * hb, nr = std::min(hb, r_hi - a);
+#ifndef B200JK_EMULATE
+            if (b >= 2) CK(cudaStreamWaitEvent(cp_stream, ev_free[b & 1], 0));
+            if (timed) CK(cudaEventRecord(blk_ev[4 * b], cp_stream));
+            CK(cudaMemcpyAsync(d_stage[b & 1], host_row(a), (size_t)nr * ld * 8, cudaMemcpyHostToDevice, cp_stream));
+            CK(cudaEventRecord(blk_ev[4 * b + 1], cp_stream));
+#else
+            memcpy(d_stage[b & 1], host_row(a), (size_t)nr * ld * 8);
+#endif
+        };
+        for (int b = 0; b < std::min(nblk, 2); b++) copy(b);
+        if (r_dev > r_lo || nblk == 0) visit(dev + (size_t)r_lo * ld, r_lo, r_dev - r_lo);
+        for (int b = 0; b < nblk; b++) {
+            const int a = r_dev + b * hb, nr = std::min(hb, r_hi - a);
+#ifndef B200JK_EMULATE
+            if (timed) CK(cudaEventRecord(blk_ev[4 * b + 2], st));
+            CK(cudaStreamWaitEvent(st, blk_ev[4 * b + 1], 0));
+            if (timed) CK(cudaEventRecord(blk_ev[4 * b + 3], st));
+#endif
+            visit(d_stage[b & 1], a, nr);
+#ifndef B200JK_EMULATE
+            CK(cudaEventRecord(ev_free[b & 1], st));
+#endif
+            if (b + 2 < nblk) copy(b + 2);
+            if (timed) bytes += (int64_t)nr * ld * 8;
+        }
+    }
+
+#ifndef B200JK_EMULATE
+    // copy and exposed copy time of the last timed walk, once its stream is synchronised
+    void read_times()
+    {
+        for (int b = 0; b < timed_blocks; b++) {
+            float tc = 0, tw = 0;
+            CK(cudaEventElapsedTime(&tc, blk_ev[4 * b], blk_ev[4 * b + 1]));
+            CK(cudaEventElapsedTime(&tw, blk_ev[4 * b + 2], blk_ev[4 * b + 3]));
+            copy_ms += tc; exposed_ms += tw;
+        }
+    }
+#endif
+};
+
+#ifndef B200JK_EMULATE
+// per-stage device timers of the last b200jk_df_jk call: mark(tag) ... mark(-1) brackets one stage with CUDA events on the
+// stream, without host synchronisation; read() adds the brackets up once the stream is synchronised
+struct StageTimer {
+    std::vector<cudaEvent_t> ev; std::vector<int> tag; size_t used = 0;
+    ~StageTimer() { for (cudaEvent_t e : ev) cudaEventDestroy(e); }
+    void start() { used = 0; tag.clear(); }
+    void mark(int t, cudaStream_t st)
+    {
+        if (used == ev.size()) { cudaEvent_t e; CK(cudaEventCreate(&e)); ev.push_back(e); }
+        CK(cudaEventRecord(ev[used++], st));
+        tag.push_back(t);
+    }
+    void read(double* ms, int* n) const
+    {
+        for (int i = 0; i < B200JK_DF_NSTAGE; i++) { ms[i] = 0; n[i] = 0; }
+        for (size_t i = 0; i + 1 < used; i++) {
+            if (tag[i] < 0) continue;
+            float t = 0;
+            CK(cudaEventElapsedTime(&t, ev[i], ev[i + 1]));
+            ms[tag[i]] += t; n[tag[i]]++;
+        }
+    }
+};
+#endif
+
 struct DFState {
     std::vector<DevShell> ash;
     int nash = 0, naux_cart = 0, naux_sph = 0, naux = 0;   // naux = rows of cderi (after lin.dep. removal)
@@ -68,14 +291,8 @@ struct DFState {
     int64_t* d_koff[NPC] = {nullptr};
     std::vector<int64_t> koff_h[NPC];
     int build_rank = 0, build_world = 1, row0 = 0, nrow = 0;   // rows [row0, row0+nrow) of the tensor live on this rank
-    double* d_cderi = nullptr;
-    // local rows [0, n_dev) live in d_cderi, rows [n_dev, nrow) in pinned host memory h_cderi; the host rows are streamed
-    // through the two device staging buffers d_stage (stage_rows rows each) once per J/K call.  n_dev == nrow when the
-    // tensor fits next to the K workspaces.
-    int n_dev = 0, stage_rows = 0;
-    double* h_cderi = nullptr;
-    double* d_stage[2] = {nullptr, nullptr};
-    int64_t stream_bytes = 0; double stream_copy_ms = 0.0, stream_exposed_ms = 0.0;   // last J/K call (b200jk_df_stream_stats)
+    double* d_cderi = nullptr;   // the local rows [0, rows.n_dev)
+    RowSplit rows;
     double omega = 0.0;
     // metric factor kept for the integral-direct J (df_jk.get_j): Cholesky L (GPU: column-major lower, emulation: row-major
     // lower) or, when the metric is not positive definite, W = diag(w)^-1/2 V^T [naux, naux_sph] row-major
@@ -105,13 +322,7 @@ struct DFState {
     // memory permits: all of them when the tensor is small or sharded over enough GPUs); the rest is cut per block into SAt
     bool sa_decided = false; int sa_np = 0, sa_ns = 0, sa_lo = 0, sa_hi = 0;
     i8g::SliceStack SAt;
-    // per-stage device timers of the last b200jk_df_jk call (CUDA events on the launching stream, read after the final sync)
-    std::vector<cudaEvent_t> tm_ev; std::vector<int> tm_tag; size_t tm_used = 0;
-    // streamed host rows: H2D copies run on cp_stream; per staged block, events at copy start / end and around the wait of
-    // the compute stream (exposed copy time); ev_free[slot] marks the compute on a staging buffer done
-    cudaStream_t cp_stream = nullptr;
-    std::vector<cudaEvent_t> sx_ev;
-    cudaEvent_t ev_free[2] = {nullptr, nullptr};
+    StageTimer timer;
 #endif
     double stage_ms[B200JK_DF_NSTAGE] = {0}; int stage_n[B200JK_DF_NSTAGE] = {0};
     // MO transforms (df_ao2mo.cuh): device ms of stage 1 and stage 2 and host ms of the last call; test cap on the output band rows
@@ -126,16 +337,8 @@ void df_free(DFState* d)
 {
     if (!d) return;
 #ifndef B200JK_EMULATE
-    for (cudaEvent_t e : d->tm_ev) cudaEventDestroy(e);
-    for (cudaEvent_t e : d->sx_ev) cudaEventDestroy(e);
-    for (cudaEvent_t e : d->ev_free) if (e) cudaEventDestroy(e);
-    if (d->cp_stream) cudaStreamDestroy(d->cp_stream);
-    if (d->h_cderi) cudaFreeHost(d->h_cderi);
     for (double* p : d->h_pin) if (p) cudaFreeHost(p);
-#else
-    free(d->h_cderi);
 #endif
-    dev_free(d->d_stage[0]); dev_free(d->d_stage[1]);
     dev_free(d->d_aprims);
     for (int l = 0; l <= LMAX; l++) { dev_free(d->d_akets[l]); dev_free(d->d_aket_off[l]); }
     dev_free(d->d_acart_sh); dev_free(d->d_acart_comp); dev_free(d->d_asph_sh); dev_free(d->d_asph_m);
@@ -538,76 +741,6 @@ static void for_each_j3c_batch(b200jk_handle h, DFState* d, double omega, stream
     dev_free(d_xc); dev_free(d_xa);
 }
 
-// ---- device / host row split ---------------------------------------------------------------------
-// bytes of int8 slices per packed row, and what the K build needs besides the tensor: the per-block slice stack and 12 GB of
-// workspaces (the reserve the slice-residency decision of df_jk_impl keeps)
-static size_t slice_row_bytes(int nao, int ns) { return (size_t)ns * nao * (((size_t)nao + 127) / 128 * 128); }
-static size_t k_reserve_bytes(int nao, int kb, int ns) { return (size_t)(kb + 1) * slice_row_bytes(nao, ns) + (12UL << 30); }
-
-// MemAvailable of /proc/meminfo in bytes (0 when it cannot be read)
-static size_t host_mem_available()
-{
-    FILE* f = fopen("/proc/meminfo", "r");
-    if (!f) return 0;
-    char line[256];
-    size_t kb = 0;
-    while (fgets(line, sizeof line, f))
-        if (sscanf(line, "MemAvailable: %zu kB", &kb) == 1) break;
-    fclose(f);
-    return kb * 1024;
-}
-
-// Decide how many of this rank's nloc rows stay in HBM and allocate d_cderi (zero-filled on request), the pinned host rows and the two
-// staging buffers.  With the automatic split (h->df_dev_rows = -1) every row stays on the device when the tensor fits next to
-// the K reserve; otherwise the device keeps as many rows as leave room for that reserve and the staging buffers.  The host
-// part is checked against MemAvailable before it is allocated; when it does not fit either, the state is freed and the call
-// fails.  Returns an empty string on success, else the error.
-static std::string plan_rows(b200jk_handle h, DFState* d, int nloc, bool zero_fill, stream_t st)
-{
-    const int nao = h->nsph;
-    const size_t rowb = (size_t)d->ncol * 8;
-    const size_t stage_cap = std::max<size_t>(1, std::min<size_t>(std::max(nloc, 1), (1UL << 30) / rowb));   // rows in 1 GiB
-    long n_dev = nloc;
-    if (h->df_dev_rows >= 0) n_dev = std::min<long>(nloc, h->df_dev_rows);
-#ifndef B200JK_EMULATE
-    else {
-        size_t freeb = 0, totb = 0;
-        CK(cudaMemGetInfo(&freeb, &totb));
-        const long n2 = (long)nao * nao;
-        const int kb = (int)std::max<long>(1, std::min<long>(std::max(nloc, 1), (2048L << 20) / (n2 * 8)));   // df_jk_impl's K block
-        const double reserve = (double)k_reserve_bytes(nao, kb, d->k_slices);
-        if ((double)nloc * rowb + reserve > (double)freeb) {
-            const double avail = (double)freeb - reserve - 2.0 * stage_cap * rowb - (double)(1UL << 30);
-            n_dev = avail > 0 ? std::min<long>(nloc, (long)(avail / rowb)) : 0;
-        }
-    }
-#endif
-    const long n_host = nloc - n_dev;
-    if (n_host > 0) {
-        const size_t hbytes = (size_t)n_host * rowb, avail = host_mem_available();
-        if (avail && (double)hbytes > 0.9 * (double)avail - (double)(2UL << 30)) {
-            char buf[320];
-            snprintf(buf, sizeof buf, "the DF tensor does not fit: %ld of its %d rows (%.1f GB) exceed the device and need pinned host "
-                     "memory, but MemAvailable is %.1f GB", n_host, nloc, hbytes / 1e9, avail / 1e9);
-            return buf;
-        }
-    }
-    d->n_dev = (int)n_dev;
-    d->d_cderi = (double*)dev_alloc((size_t)std::max<long>(n_dev, 1) * rowb);
-    if (zero_fill) dev_zero(d->d_cderi, (size_t)std::max<long>(n_dev, 1) * rowb, st);
-    if (n_host > 0) {
-        d->stage_rows = (int)std::min<long>((long)stage_cap, n_host);
-#ifndef B200JK_EMULATE
-        CK(cudaHostAlloc((void**)&d->h_cderi, (size_t)n_host * rowb, cudaHostAllocDefault));
-#else
-        d->h_cderi = (double*)malloc((size_t)n_host * rowb);
-        if (!d->h_cderi) throw std::runtime_error("host rows of the DF tensor: out of memory");
-#endif
-        for (double*& s : d->d_stage) s = (double*)dev_alloc((size_t)d->stage_rows * rowb);
-    }
-    return "";
-}
-
 // Pair screening of the tensor's columns: the Schwarz bound q = sqrt((ab|ab)) of every device shell pair for the tensor's own
 // operator (SchwarzSphFn: the reference's normalisation, per segment of a general contraction, as b200jk_set_screening computes
 // it, but on a copy of the pair list so that the 4-center screening state of the handle is left as it is).  A packed column
@@ -822,7 +955,8 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
 
         // ---- rows of the metric transform owned by this rank: T[nloc][nas] (rows of L^-1, or of W = diag(w)^-1/2 V^T)
         const int bw = h->shard_world, br = h->shard_rank;
-        const int r_lo = (int)((long)nkeep * br / bw), r_hi = (int)((long)nkeep * (br + 1) / bw);
+        int r_lo, r_hi;
+        shard_range(nkeep, br, bw, r_lo, r_hi);
         const int nloc = r_hi - r_lo;
         d->build_rank = br; d->build_world = bw; d->row0 = r_lo; d->nrow = nloc;
         double* d_T = (double*)dev_alloc((size_t)std::max(nloc, 1) * nas * 8);
@@ -868,13 +1002,13 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
         const long ncol = d->ncol;   // row length: every packed column, or the kept ones under pair screening
         const int64_t bcols = std::min<int64_t>(std::max<int64_t>(4096, (int64_t)((3ULL << 30) / ((size_t)d->naux_cart * 8))) + 128, d->rowlen);
         double* d_ybatch = (double*)dev_alloc((size_t)std::max(nloc, 1) * (size_t)bcols * 8);
-        const std::string split_err = plan_rows(h, d, nloc, true, st);
+        const std::string split_err = d->rows.plan(h, nloc, ncol, d->k_slices, true, &d->d_cderi, st);
         if (!split_err.empty()) {
             dev_free(d_T); dev_free(d_ybatch); dev_free(d_j2c_cart);
             df_free(d); h->df = nullptr;
             throw std::runtime_error(split_err);
         }
-        const int n_dev = d->n_dev, n_host = nloc - n_dev;
+        const int n_dev = d->rows.n_dev, n_host = nloc - n_dev;
         // rows of the tensor from the rows Trows[nr][nas] of the metric transform into out[nr][ncol] (zero-filled); under pair
         // screening only the kept shell pairs are integrated and their columns written through col_of
         const bool kept = d->pair_screened;
@@ -913,7 +1047,7 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
         if (n_host > 0) {
             // host rows in blocks as large as the device memory left over allows (the K reserve is not in use yet); the 3-center
             // integrals are recomputed once per block (d_ybatch holds nloc >= hb rows)
-            long hb = d->stage_rows;
+            long hb = d->rows.stage_rows;
 #ifndef B200JK_EMULATE
             size_t freeb = 0, totb = 0;
             CK(cudaMemGetInfo(&freeb, &totb));
@@ -926,7 +1060,7 @@ static int df_build_impl(b200jk_handle h, const int32_t* aux_atm, int aux_natm, 
                 const int nr = (int)std::min<long>(hb, nloc - a);
                 dev_zero(d_blk, (size_t)nr * ncol * 8, st);
                 fill_rows(d_T + (size_t)a * nas, nr, d_blk);
-                d2h(d->h_cderi + (size_t)(a - n_dev) * ncol, d_blk, (size_t)nr * ncol * 8, st);
+                d2h(d->rows.host_row(a), d_blk, (size_t)nr * ncol * 8, st);
             }
 #ifndef B200JK_EMULATE
             CK(cudaStreamSynchronize(st));
@@ -1145,13 +1279,15 @@ extern "C" int b200jk_df_set_cderi(b200jk_handle h, const double* cderi, int nau
         d->ncol = d->npair;     // an assigned tensor stays dense: pair screening applies to tensors built here
         d->naux = naux;
         const int bw = h->shard_world, br = h->shard_rank;
-        const int r_lo = (int)((long)naux * br / bw), r_hi = (int)((long)naux * (br + 1) / bw);
+        int r_lo, r_hi;
+        shard_range(naux, br, bw, r_lo, r_hi);
         d->build_rank = br; d->build_world = bw; d->row0 = r_lo; d->nrow = r_hi - r_lo;
-        const std::string split_err = plan_rows(h, d, d->nrow, false, st);
+        const std::string split_err = d->rows.plan(h, d->nrow, d->ncol, d->k_slices, false, &d->d_cderi, st);
         if (!split_err.empty()) { df_free(d); h->df = nullptr; throw std::runtime_error(split_err); }
-        if (d->n_dev > 0) h2d(d->d_cderi, cderi + (size_t)r_lo * d->npair, (size_t)d->n_dev * d->npair * 8, st);
-        if (d->nrow > d->n_dev)
-            memcpy(d->h_cderi, cderi + (size_t)(r_lo + d->n_dev) * d->npair, (size_t)(d->nrow - d->n_dev) * d->npair * 8);
+        const int n_dev = d->rows.n_dev;
+        if (n_dev > 0) h2d(d->d_cderi, cderi + (size_t)r_lo * d->npair, (size_t)n_dev * d->npair * 8, st);
+        if (d->nrow > n_dev)
+            memcpy(d->rows.host_row(n_dev), cderi + (size_t)(r_lo + n_dev) * d->npair, (size_t)(d->nrow - n_dev) * d->npair * 8);
 #ifndef B200JK_EMULATE
         CK(cudaStreamSynchronize(st));
 #endif
@@ -1190,18 +1326,19 @@ extern "C" int b200jk_df_get_cderi_cols(b200jk_handle h, double* out, const int6
         std::vector<long> pos(cols, cols + ncols);     // positions in the stored rows
         if (d->d_col_of)
             for (long& p : pos) p = d->col_of_h[(size_t)p];
-        if (d->n_dev > 0) {
+        const int n_dev = d->rows.n_dev;
+        if (n_dev > 0) {
             long* d_cols = (long*)dev_alloc((size_t)ncols * 8);
-            double* d_out = (double*)dev_alloc((size_t)d->n_dev * ncols * 8);
+            double* d_out = (double*)dev_alloc((size_t)n_dev * ncols * 8);
             h2d(d_cols, pos.data(), (size_t)ncols * 8);
             GatherColsFn g{d->d_cderi, d_cols, d_out, d->ncol, ncols};
-            launch_1d((long)d->n_dev * ncols, g, 0);
-            d2h(out, d_out, (size_t)d->n_dev * ncols * 8);
+            launch_1d((long)n_dev * ncols, g, 0);
+            d2h(out, d_out, (size_t)n_dev * ncols * 8);
             dev_sync();
             dev_free(d_cols); dev_free(d_out);
         }
-        for (long r = 0; r < d->nrow - d->n_dev; r++)      // rows in pinned host memory
-            for (int c = 0; c < ncols; c++) out[(d->n_dev + r) * ncols + c] = pos[c] >= 0 ? d->h_cderi[r * d->ncol + pos[c]] : 0.0;
+        for (long r = n_dev; r < d->nrow; r++)      // rows in pinned host memory
+            for (int c = 0; c < ncols; c++) out[r * ncols + c] = pos[c] >= 0 ? d->rows.host_row(r)[pos[c]] : 0.0;
     } catch (std::exception& e) { set_err(h, e.what()); return 2; }
     return 0;
 }
@@ -1216,14 +1353,7 @@ extern "C" int b200jk_df_get_cderi(b200jk_handle h, double* out, int r0, int nr)
         if (r0 < 0 || nr < 0 || r0 + nr > d->nrow) throw std::runtime_error("row range out of bounds (rows are local to this rank)");
         const long ld = d->ncol;
         std::vector<double> packed(d->d_col_of ? (size_t)nr * ld : 0);
-        double* dst = d->d_col_of ? packed.data() : out;    // the stored rows, expanded below when pair-screened
-        const int nd = std::max(0, std::min(r0 + nr, d->n_dev) - r0);     // rows in HBM, then rows in pinned host memory
-        if (nd > 0) {
-            d2h(dst, d->d_cderi + (size_t)r0 * ld, (size_t)nd * ld * 8);
-            dev_sync();
-        }
-        if (nr > nd)
-            memcpy(dst + (size_t)nd * ld, d->h_cderi + (size_t)(r0 + nd - d->n_dev) * ld, (size_t)(nr - nd) * ld * 8);
+        d->rows.read(d->d_col_of ? packed.data() : out, d->d_cderi, r0, nr);   // the stored rows, expanded below when pair-screened
         if (d->d_col_of) {
             memset(out, 0, (size_t)nr * d->npair * 8);
             for (long r = 0; r < nr; r++)
@@ -1231,6 +1361,295 @@ extern "C" int b200jk_df_get_cderi(b200jk_handle h, double* out, int r0, int nr)
         }
     } catch (std::exception& e) { set_err(h, e.what()); return 2; }
     return 0;
+}
+
+// ---- J/K from the tensor ------------------------------------------------------------------------
+// copies between the J/K workspaces and the caller's arrays, in host memory or, for b200jk_df_jk_device, on the device
+static void copy_in(void* dst, const void* src, size_t n, bool on_device, stream_t st) { if (on_device) d2d(dst, src, n, st); else h2d(dst, src, n, st); }
+static void copy_out(void* dst, const void* src, size_t n, bool on_device, stream_t st) { if (on_device) d2d(dst, src, n, st); else d2h(dst, src, n, st); }
+
+// one J/K call: its shape and options, shared by the J part and the K engines
+struct JKCall {
+    DFState* d;
+    int nao, n_dm; long n2;
+    long ld; const int* col_of;   // stored row length: npair, or the kept columns of a pair-screened tensor (col_of != nullptr)
+    int naux;                     // rows held locally (stride of rho)
+    int r_lo, kb;                 // first row of this rank's range; rows per K block
+    bool use_occ; int nocc, ncol; // K from the orbitals (ncol = nocc) or from the density itself (ncol = nao)
+    bool k_sym;                   // K is symmetric: the int8 engine computes its upper triangle, mirrored at the end
+    bool tc;                      // the int8-slice engine (k_mode 1), else the FP64 one
+    bool on_device;
+    stream_t st;
+    uint64_t launches;
+};
+
+// J, after the rows: unpack J~ and hand it to the caller
+static void finish_j(JKCall& c, double* vj)
+{
+    UnpackTrilFn uf{c.d->d_vjtril, c.d->d_vj, c.nao, c.ld, c.col_of};     // a dropped pair gets J = 0
+    launch_1d((long)c.n_dm * c.n2, uf, c.st); c.launches++;
+    copy_out(vj, c.d->d_vj, (size_t)c.n_dm * c.n2 * 8, c.on_device, c.st);
+}
+
+// J, before the walk: the packed density and zeroed accumulators
+static void j_prepare(JKCall& c)
+{
+    DFState* d = c.d;
+    DmTrilFn tf{d->d_dm, d->d_dmtril, c.nao, c.ld, d->d_pk_of};     // pair screening: the kept columns only
+    launch_1d((long)c.n_dm * c.ld, tf, c.st); c.launches++;
+    dev_zero(d->d_vjtril, (size_t)c.n_dm * c.ld * 8, c.st);
+    dev_zero(d->d_rho, (size_t)c.n_dm * c.naux * 8, c.st);
+}
+
+#ifndef B200JK_EMULATE
+// J of the rows [r0, r0 + nr) at src (row r0 first): rho, then J~ += rho . rows — two streaming passes, both HBM-bound
+static void j_rows(JKCall& c, const double* src, int r0, int nr)
+{
+    DFState* d = c.d;
+    d->timer.mark(B200JK_DF_STAGE_J_RHO, c.st);
+    rows_dot(src, nr, c.ld, d->d_dmtril, c.ld, d->d_rho + r0, c.naux, c.n_dm, c.st);
+    c.launches += (nr + 32768L * DFJ_R - 1) / (32768L * DFJ_R);
+    d->timer.mark(B200JK_DF_STAGE_J_ACC, c.st);
+    cols_acc(src, nr, c.ld, d->d_rho + r0, c.naux, d->d_vjtril, c.ld, c.n_dm, c.st);
+    c.launches++;
+    d->timer.mark(-1, c.st);
+}
+
+// Keep the int8 slices of as many packed device rows of this rank's range as fit (7 B per unpacked element) resident in SA:
+// all of them when the tensor is small or sharded over enough GPUs; otherwise a leading part, the rest being re-cut block by
+// block every call.  Decided again when the range, the slice count or the caps of b200jk_df_set_kblock change.
+static void resident_slices(JKCall& c, int r_hi)
+{
+    DFState* d = c.d;
+    if (d->sa_decided && d->sa_ns == d->k_slices && d->sa_lo == c.r_lo && d->sa_hi == r_hi) return;
+    const int nao = c.nao;
+    size_t freeb = 0, totb = 0;
+    CK(cudaMemGetInfo(&freeb, &totb));
+    freeb += d->SA.cap;                                         // an earlier stack of this handle is reused
+    const size_t per_row = slice_row_bytes(nao, d->k_slices);
+    const size_t reserve = k_reserve_bytes(nao, c.kb, d->k_slices);   // the per-block stack + workspaces allocated later
+    const long nloc = d->rows.dev_end(c.r_lo, r_hi) - c.r_lo;   // only rows in HBM can be resident
+    long np = 0;
+    if (freeb * 0.85 > (double)reserve) np = (long)((freeb * 0.85 - (double)reserve) / (double)per_row);
+    if (np >= nloc) np = nloc;
+    else if (np < nloc / 10) np = 0;                            // not worth a second code path
+    if (d->np_max >= 0) np = std::min(np, (long)d->np_max);
+    while (np > 0 && (size_t)np * nao >= (1UL << 31) - 256) np--;   // row index of the stack is an int
+    d->sa_np = (int)np;
+    if (np > 0) {
+        const size_t kp = ((size_t)nao + 127) / 128 * 128, rows_p = (size_t)np * nao, rp = ((rows_p + 255) / 256) * 256;
+        d->SA.alloc((int)rows_p, nao, d->k_slices);
+        CK(cudaMemsetAsync(d->SA.q, 0, (size_t)d->k_slices * rp * kp, c.st));
+        CK(cudaMemsetAsync(d->SA.E, 0, rp * 4, c.st));
+        i8g::split_packed_into(d->SA, 0, d->d_cderi + (size_t)c.r_lo * c.ld, c.ld, nao, (int)np, d->d_rowexp + (size_t)c.r_lo * nao, c.st, c.col_of);
+    }
+    d->sa_decided = true; d->sa_ns = d->k_slices; d->sa_lo = c.r_lo; d->sa_hi = r_hi;
+}
+
+// buffers of the int8 engine: stage 2 in one K range needs pairs(<=ns) * K * 64*64 <= 2^31 - 1 (gemm_ar_acc splits K further
+// where this does not hold; gemm_ar rejects a stage 1 whose nao breaks the bound); the slice exponents of the device rows are
+// made once (host rows: per staged block, every call)
+static void i8_prepare(JKCall& c, int r_hi)
+{
+    DFState* d = c.d;
+    const int nao = c.nao;
+    const int kmax = (int)(((1L << 31) - 1) / (4096L * d->k_slices));
+    c.kb = std::max(1, std::min(c.kb, kmax / ((c.ncol + 15) & ~15)));   // stage 2 contracts over (P, i) with i padded to 16
+    if ((size_t)c.kb * c.ncol * nao > d->y2_cap) { dev_free(d->d_Y2); d->y2_cap = (size_t)c.kb * c.ncol * nao; d->d_Y2 = (double*)dev_alloc(d->y2_cap * 8); }
+    if ((size_t)c.ncol * nao > d->occT_cap) { dev_free(d->d_occT); d->occT_cap = (size_t)c.ncol * nao; d->d_occT = (double*)dev_alloc(d->occT_cap * 8); }
+    if (!d->d_rowexp) {
+        d->d_rowexp = (int*)dev_alloc((size_t)std::max(d->nrow, 1) * nao * 4);
+        d->d_rownorm2 = (float*)dev_alloc((size_t)std::max(d->nrow, 1) * nao * 4);
+        d->d_cmax2 = (double*)dev_alloc(8);
+        if (d->rows.n_dev == d->nrow || d->rows.n_dev > 0)
+            i8g::packed_rowexp(d->d_cderi, c.ld, nao, d->rows.n_dev, d->d_rowexp, d->d_rownorm2, c.st, c.col_of);
+    }
+    resident_slices(c, r_hi);
+}
+
+// int8-slice engine on the rows [r0, r0 + nr) at src: the occupied-orbital algorithm when the density carries its orbitals
+// (pyscf/df/df_jk.py:339-357), else the general-density algorithm (df_jk.py:382-408) with the density itself as the right
+// factor: Y[nu,(P,k)] = sum_mu A_P[nu,mu] D[mu,k], K[i,l] = sum_(P,k) Y[i,(P,k)] A_P[l,k] — the same two int8-slice GEMM
+// stages, no cuBLAS
+static void k_block_i8(JKCall& c, const double* src, int r0, int nr)
+{
+    static const bool fuse_y = getenv("B200JK_NO_YFUSE") == nullptr;   // stage 1 cuts the int8 slices of Y itself
+    DFState* d = c.d;
+    const int nao = c.nao, ncol = c.ncol, ns = d->k_slices;
+    const cudaStream_t st = c.st;
+    const bool resident = r0 - c.r_lo + nr <= d->sa_np;
+    if (!resident) {    // slices of this block straight from the packed rows
+        d->timer.mark(B200JK_DF_STAGE_K_SLICE, st);
+        i8g::split_packed(d->SAt, src, c.ld, nao, nr, d->d_rowexp + (size_t)r0 * nao, ns, st, c.col_of);
+        d->timer.mark(-1, st);
+        c.launches++;
+    }
+    if (!c.use_occ) {   // general density: the block once more as nao long rows G[l][(P,k)] = A_P[l][k]
+        d->timer.mark(B200JK_DF_STAGE_K_SLICE, st);
+        // same (P, k) column layout as Y: k padded to 16 when stage 1 cuts the slices of Y itself
+        const int gcol = fuse_y ? ((nao + 15) & ~15) : nao;
+        UnpackLongFn ul{src, d->d_A, nao, c.ld, 0, (long)nr * gcol, gcol, c.col_of};
+        launch_1d((long)nao * nr * gcol, ul, st);
+        i8g::split_rows(d->SG, d->d_A, (long)nr * gcol, nao, nr * gcol, ns, st);
+        d->timer.mark(-1, st);
+        c.launches += 2;
+    }
+    const i8g::SliceStack& A = resident ? d->SA : d->SAt;
+    const int a0 = resident ? (r0 - c.r_lo) * nao : 0;
+    for (int s = 0; s < c.n_dm; s++) {
+        // Y2[nu][(P,i)] = sum_mu A_P[nu,mu] Ct[i,mu] ; K += Y2 Y2^T (upper triangle)
+        if (r0 == c.r_lo || c.n_dm > 1) {
+            // right factor of stage 1 as rows [ncol][nao]: C~^T, or D^T for the general-density algorithm
+            TransposeFn tr{c.use_occ ? d->d_occ + (size_t)s * nao * c.nocc : d->d_dm + (size_t)s * c.n2, d->d_occT, nao, ncol};
+            launch_1d((long)nao * ncol, tr, st);
+            i8g::split_rows(d->SC, d->d_occT, nao, ncol, nao, ns, st); c.launches += 2;
+            i8g::colnorm_max(d->d_occT, nao, ncol, nao, d->d_cmax2, st);
+        }
+        d->timer.mark(B200JK_DF_STAGE_K_GEMM1, st);
+        if (fuse_y) {
+            // the row exponents of Y are bounded BEFORE the GEMM (||A_P[nu,:]||_2 max_i ||C~_i||_2), fp64 Y is never written
+            const int ncolp = (ncol + 15) & ~15;
+            i8g::y_prepare(d->SY, nao, nr, ncolp, ns, d->d_rownorm2 + (size_t)r0 * nao, d->d_cmax2, st);
+            i8g::gemm_ar(A, a0, nr * nao, d->SC, nullptr, 0, nao, st, nullptr, &d->SY, ncolp);
+            d->timer.mark(B200JK_DF_STAGE_K_SLICE, st);
+        } else {
+            // stage 1 leaves the row maxima of Y behind (GemmParams::rowmax): the slicing of Y is one pass
+            const bool premax = (long)nr * ncol >= 8192;
+            if (premax) i8g::split_rows_prepare(d->SY, nao, nr * ncol, ns, st);
+            i8g::gemm_ar(A, a0, nr * nao, d->SC, d->d_Y2, (long)nr * ncol, nao, st, premax ? d->SY.maxbits : nullptr);
+            d->timer.mark(B200JK_DF_STAGE_K_SLICE, st);
+            if (premax) i8g::split_rows_premax(d->SY, d->d_Y2, (long)nr * ncol, nao, nr * ncol, ns, st);
+            else i8g::split_rows(d->SY, d->d_Y2, (long)nr * ncol, nao, nr * ncol, ns, st);
+        }
+        d->timer.mark(B200JK_DF_STAGE_K_GEMM2, st);
+        // K += Y Y^T (orbitals) or Y G^T (general density; only its upper triangle when D, hence K, is symmetric)
+        i8g::gemm_ar_acc(d->SY, c.use_occ ? d->SY : d->SG, d->d_vk + (size_t)s * c.n2, nao, c.k_sym, st);
+        d->timer.mark(-1, st);
+        c.launches += 3;
+    }
+}
+
+// cuBLAS DGEMM engine (k_mode 0, FP64 pipe) on the rows at src: the yardstick the int8 engine is tested and measured against
+static void k_block_dgemm(JKCall& c, const double* src, int nr)
+{
+    DFState* d = c.d;
+    const int nao = c.nao, nocc = c.nocc;
+    const long n2 = c.n2;
+    UnpackFn up{src, d->d_A, nao, c.ld, 0, c.col_of};
+    launch_1d((long)nr * n2, up, c.st); c.launches++;
+    const double one = 1.0, zero = 0.0;
+    for (int s = 0; s < c.n_dm; s++) {
+        if (c.use_occ) {
+            // Y_P (col-major [nao, nocc]) = A_P * Ctilde ; buffers: occ row-major [nao,nocc] == col-major [nocc,nao]
+            CKB(cublasDgemmStridedBatched(d->cublas, CUBLAS_OP_N, CUBLAS_OP_T, nao, nocc, nao, &one, d->d_A, nao, n2,
+                                          d->d_occ + (size_t)s * nao * nocc, nocc, 0, &zero, d->d_Y, nao,
+                                          (long long)nao * nocc, nr));
+            // K += Z Z^T, Z = [nao, nr*nocc]
+            CKB(cublasDgemm(d->cublas, CUBLAS_OP_N, CUBLAS_OP_T, nao, nao, nr * nocc, &one, d->d_Y, nao, d->d_Y, nao, &one,
+                            d->d_vk + (size_t)s * n2, nao));
+        } else {
+            // general dm: T_P = A_P * Dbuf (col-major view), K += sum_P T_P * A_P
+            CKB(cublasDgemmStridedBatched(d->cublas, CUBLAS_OP_N, CUBLAS_OP_N, nao, nao, nao, &one, d->d_A, nao, n2,
+                                          d->d_dm + (size_t)s * n2, nao, 0, &zero, d->d_Y, nao, n2, nr));
+            CKB(cublasDgemm(d->cublas, CUBLAS_OP_N, CUBLAS_OP_T, nao, nao, nr * nao, &one, d->d_Y, nao, d->d_A, nao, &one,
+                            d->d_vk + (size_t)s * n2, nao));
+        }
+        c.launches += 2;
+    }
+}
+
+static void k_block(JKCall& c, const double* src, int r0, int nr)
+{
+    if (c.tc) k_block_i8(c, src, r0, nr);
+    else k_block_dgemm(c, src, nr);
+}
+#else
+static void j_rows(JKCall& c, const double* src, int, int nr)
+{
+    DFState* d = c.d;
+    const long ld = c.ld;
+    for (int s = 0; s < c.n_dm; s++)
+        for (int r = 0; r < nr; r++) {
+            double acc = 0;
+            for (long t = 0; t < ld; t++) acc += src[(size_t)r * ld + t] * d->d_dmtril[(size_t)s * ld + t];
+            for (long t = 0; t < ld; t++) d->d_vjtril[(size_t)s * ld + t] += acc * src[(size_t)r * ld + t];
+        }
+}
+
+// C[m][n] = A[m][k] B (B[k][n], or B[n][k] transposed when bt), or C += A B when add: each element summed in k order
+static void host_mm(const double* A, const double* B, double* C, int m, int n, int k, bool bt, bool add)
+{
+    for (int i = 0; i < m; i++)
+        for (int l = 0; l < n; l++) {
+            double acc = 0;
+            for (int j = 0; j < k; j++) acc += A[(size_t)i * k + j] * (bt ? B[(size_t)l * k + j] : B[(size_t)j * n + l]);
+            C[(size_t)i * n + l] = add ? C[(size_t)i * n + l] + acc : acc;
+        }
+}
+
+// the emulation's engine (tests only), per unpacked row A_P: the occupied-orbital algebra of the int8 engine, Y = A_P C~ and
+// K += Y Y^T, so that the host-side handling of mo_coeff / mo_occ is exercised on the CPU as well; else K += A_P D A_P (O(N^4))
+static void k_block(JKCall& c, const double* src, int, int nr)
+{
+    DFState* d = c.d;
+    const int nao = c.nao, nocc = c.nocc;
+    UnpackFn up{src, d->d_A, nao, c.ld, 0, c.col_of};
+    launch_1d((long)nr * c.n2, up, c.st); c.launches++;
+    std::vector<double> Y((size_t)nao * c.ncol);
+    for (int s = 0; s < c.n_dm; s++)
+        for (int r = 0; r < nr; r++) {
+            const double* A = d->d_A + (size_t)r * c.n2;
+            double* K = d->d_vk + (size_t)s * c.n2;
+            if (c.use_occ) {
+                host_mm(A, d->d_occ + (size_t)s * nao * nocc, Y.data(), nao, nocc, nao, false, false);
+                host_mm(Y.data(), Y.data(), K, nao, nao, nocc, true, true);
+            } else {
+                host_mm(A, d->d_dm + (size_t)s * c.n2, Y.data(), nao, nao, nao, false, false);
+                host_mm(Y.data(), A, K, nao, nao, nao, false, true);
+            }
+        }
+}
+#endif
+
+// K, before the walk: the workspaces (rows of A padded to 16 columns for the general-density G operand; Y for the FP64 engine
+// only), the orbitals, a zeroed K and the int8 engine's own buffers
+static void k_prepare(JKCall& c, const double* occ, int r_hi)
+{
+    DFState* d = c.d;
+    const int nao = c.nao;
+    if ((size_t)c.kb > d->ws_rows || (size_t)c.ncol > d->ws_nocc || (size_t)c.n_dm > d->ws_occ_ndm) {
+        dev_free(d->d_A); dev_free(d->d_Y); dev_free(d->d_occ);
+        d->d_A = (double*)dev_alloc((size_t)c.kb * nao * ((nao + 15) & ~15) * 8);
+        d->d_Y = (d->k_mode == 1) ? nullptr : (double*)dev_alloc((size_t)c.kb * c.ncol * nao * 8);
+        d->d_occ = (double*)dev_alloc((size_t)c.n_dm * nao * c.ncol * 8);
+        d->ws_rows = c.kb; d->ws_nocc = c.ncol; d->ws_occ_ndm = c.n_dm;
+    }
+    if (c.use_occ) copy_in(d->d_occ, occ, (size_t)c.n_dm * nao * c.nocc * 8, c.on_device, c.st);
+    dev_zero(d->d_vk, (size_t)c.n_dm * c.n2 * 8, c.st);
+#ifndef B200JK_EMULATE
+    if (c.tc) i8_prepare(c, r_hi);
+#endif
+}
+
+// K of the rows [r0, r0 + nr) at src in blocks of kb rows; staged host rows first get their slice exponents
+static void k_rows(JKCall& c, const double* src, int r0, int nr)
+{
+#ifndef B200JK_EMULATE
+    DFState* d = c.d;
+    if (c.tc && nr > 0 && r0 >= d->rows.n_dev) {
+        i8g::packed_rowexp(src, c.ld, c.nao, nr, d->d_rowexp + (size_t)r0 * c.nao, d->d_rownorm2 + (size_t)r0 * c.nao, c.st, c.col_of);
+        c.launches++;
+    }
+#endif
+    for (int q = 0; q < nr; q += c.kb) k_block(c, src + (size_t)q * c.ld, r0 + q, std::min(c.kb, nr - q));
+}
+
+// multi-GPU: this rank contracts only the local rows [r_lo, r_hi) and returns partial J/K
+static void local_range(b200jk_handle h, const DFState* d, int& r_lo, int& r_hi)
+{
+    if (d->build_world == h->shard_world && d->build_rank == h->shard_rank) { r_lo = 0; r_hi = d->nrow; }
+    else if (d->build_world == 1) shard_range(d->nrow, h->shard_rank, h->shard_world, r_lo, r_hi);
+    else throw std::runtime_error("the tensor was built for a different shard; call b200jk_df_build again after b200jk_set_shard");
 }
 
 static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, const double* occ, int nocc, int hermi,
@@ -1243,402 +1662,52 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
         if (nao != h->nsph) throw std::runtime_error("nao does not match the basis of this handle");
         if (n_dm < 1) throw std::runtime_error("n_dm < 1");
         auto t0 = std::chrono::steady_clock::now();
-        const long npair = d->npair, n2 = (long)nao * nao;
-        // row length of the stored tensor: npair, or the kept columns of a pair-screened tensor (col_of: packed index -> column)
-        const long ld = d->ncol;
-        const int* col_of = d->d_col_of;
-        const int naux = std::max(d->nrow, 1);   // rows held locally
-        // multi-GPU: this rank contracts only its auxiliary rows [r_lo, r_hi) and returns partial J/K
-        int r_lo, r_hi;   // LOCAL row indices into d_cderi
-        if (d->build_world == h->shard_world && d->build_rank == h->shard_rank) { r_lo = 0; r_hi = d->nrow; }
-        else if (d->build_world == 1) { r_lo = (int)((long)d->nrow * h->shard_rank / h->shard_world); r_hi = (int)((long)d->nrow * (h->shard_rank + 1) / h->shard_world); }
-        else throw std::runtime_error("the tensor was built for a different shard; call b200jk_df_build again after b200jk_set_shard");
-        // rows [r_lo, r_dev) are in d_cderi, rows [r_dev, r_hi) in pinned host memory: streamed through the staging buffers
-        const int r_dev = std::max(r_lo, std::min(r_hi, d->n_dev));
-        const bool streamed = r_dev < r_hi;
+        int r_lo, r_hi;
+        local_range(h, d, r_lo, r_hi);
 #ifndef B200JK_EMULATE
         CK(cudaSetDevice(h->device));
         cudaStream_t st = h->stream;
         CKB(cublasSetStream(d->cublas, st));
+        const bool tc = d->k_mode == 1;
 #else
         stream_t st = 0;
+        const bool tc = false;     // the emulation runs its host engine
 #endif
-        // rows per block: the block is read twice (rho, then J) and should stay in L2; K unpacks it to nao^2
-        int rb = (int)std::max<long>(1, std::min<long>(naux, (40L << 20) / (npair * 8)));
-        int kb = (int)std::max<long>(1, std::min<long>(naux, (2048L << 20) / (n2 * 8)));
-        if (d->kb_max > 0) kb = std::min(kb, d->kb_max);
+        const bool use_occ = (occ != nullptr && nocc > 0);
+        JKCall c{d, nao, n_dm, (long)nao * nao, d->ncol, d->d_col_of, std::max(d->nrow, 1), r_lo, k_block_rows(nao, d->nrow),
+                 use_occ, nocc, use_occ ? nocc : nao, use_occ || hermi == 1, tc, on_device, st, 0};
+        if (d->kb_max > 0) c.kb = std::min(c.kb, d->kb_max);
         if ((size_t)n_dm > d->ws_ndm) {
             for (double** p : {&d->d_dmtril, &d->d_rho, &d->d_vjtril, &d->d_dm, &d->d_vk, &d->d_vj}) { dev_free(*p); *p = nullptr; }
-            d->d_dmtril = (double*)dev_alloc((size_t)n_dm * ld * 8);
-            d->d_vjtril = (double*)dev_alloc((size_t)n_dm * ld * 8);
-            d->d_rho = (double*)dev_alloc((size_t)n_dm * naux * 8);
-            d->d_dm = (double*)dev_alloc((size_t)n_dm * n2 * 8);
-            d->d_vk = (double*)dev_alloc((size_t)n_dm * n2 * 8);
-            d->d_vj = (double*)dev_alloc((size_t)n_dm * n2 * 8);
+            d->d_dmtril = (double*)dev_alloc((size_t)n_dm * c.ld * 8);
+            d->d_vjtril = (double*)dev_alloc((size_t)n_dm * c.ld * 8);
+            d->d_rho = (double*)dev_alloc((size_t)n_dm * c.naux * 8);
+            d->d_dm = (double*)dev_alloc((size_t)n_dm * c.n2 * 8);
+            d->d_vk = (double*)dev_alloc((size_t)n_dm * c.n2 * 8);
+            d->d_vj = (double*)dev_alloc((size_t)n_dm * c.n2 * 8);
             d->ws_ndm = n_dm;
         }
-        if (!on_device) h2d(d->d_dm, dm, (size_t)n_dm * n2 * 8, st);
-        else {
-#ifndef B200JK_EMULATE
-            CK(cudaMemcpyAsync(d->d_dm, dm, (size_t)n_dm * n2 * 8, cudaMemcpyDeviceToDevice, st));
-#endif
-        }
-        uint64_t launches = 0;
+        copy_in(d->d_dm, dm, (size_t)n_dm * c.n2 * 8, on_device, st);
 #ifndef B200JK_EMULATE
         CK(cudaEventRecord(h->ev0, st));
-        d->tm_used = 0; d->tm_tag.clear();
-        // mark(tag) ... mark(-1) brackets one stage on the stream; no host synchronisation
-        auto mark = [&](int tag) {
-            if (d->tm_used == d->tm_ev.size()) { cudaEvent_t e; CK(cudaEventCreate(&e)); d->tm_ev.push_back(e); }
-            CK(cudaEventRecord(d->tm_ev[d->tm_used++], st));
-            d->tm_tag.push_back(tag);
-        };
-#else
-        auto mark = [&](int) {};
+        d->timer.start();
 #endif
-        // ---- host rows: staged blocks of hb rows, block b in staging buffer b & 1.  Blocks 0 and 1 are copied while the
-        //      device rows are contracted; block b + 2 is copied once the compute stream is done with block b.
-        const int hb = streamed ? (d->kb_max > 0 ? std::min(d->stage_rows, d->kb_max) : d->stage_rows) : 0;
-        const int nblk = streamed ? (r_hi - r_dev + hb - 1) / hb : 0;
-        d->stream_bytes = 0; d->stream_copy_ms = 0.0; d->stream_exposed_ms = 0.0;
-        auto blk_rows = [&](int b, int& a, int& nr) { a = r_dev + b * hb; nr = std::min(hb, r_hi - a); };
-#ifndef B200JK_EMULATE
-        if (streamed) {
-            if (!d->cp_stream) {
-                CK(cudaStreamCreateWithFlags(&d->cp_stream, cudaStreamNonBlocking));
-                for (cudaEvent_t& e : d->ev_free) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            }
-            while (d->sx_ev.size() < 4 * (size_t)nblk) { cudaEvent_t e; CK(cudaEventCreate(&e)); d->sx_ev.push_back(e); }
-            CK(cudaStreamWaitEvent(d->cp_stream, h->ev0, 0));     // the copies start inside the bracket of this call
-        }
-        auto issue_copy = [&](int b) {
-            int a, nr;
-            blk_rows(b, a, nr);
-            if (b >= 2) CK(cudaStreamWaitEvent(d->cp_stream, d->ev_free[b & 1], 0));
-            CK(cudaEventRecord(d->sx_ev[4 * b], d->cp_stream));
-            CK(cudaMemcpyAsync(d->d_stage[b & 1], d->h_cderi + (size_t)(a - d->n_dev) * ld, (size_t)nr * ld * 8,
-                               cudaMemcpyHostToDevice, d->cp_stream));
-            CK(cudaEventRecord(d->sx_ev[4 * b + 1], d->cp_stream));
-        };
-#else
-        auto issue_copy = [&](int b) {
-            int a, nr;
-            blk_rows(b, a, nr);
-            memcpy(d->d_stage[b & 1], d->h_cderi + (size_t)(a - d->n_dev) * ld, (size_t)nr * ld * 8);
-        };
-#endif
-        for (int b = 0; b < std::min(nblk, 2); b++) issue_copy(b);
-        auto finish_j = [&]() {
-            UnpackTrilFn uf{d->d_vjtril, d->d_vj, nao, ld, col_of};     // a dropped pair gets J = 0
-            launch_1d((long)n_dm * n2, uf, st); launches++;
-            if (!on_device) d2h(vj, d->d_vj, (size_t)n_dm * n2 * 8, st);
-            else {
-#ifndef B200JK_EMULATE
-                CK(cudaMemcpyAsync(vj, d->d_vj, (size_t)n_dm * n2 * 8, cudaMemcpyDeviceToDevice, st));
-#endif
-            }
-        };
-#ifndef B200JK_EMULATE
-        const long seglen = 16384;   // 128 KiB of a row per CTA
-        const unsigned nseg = (unsigned)((ld + seglen - 1) / seglen);
-        // J of the rows [r0, r0 + nr) at src (row r0 first): rho, then J~ += rho . rows
-        auto j_rows = [&](const double* src, int r0, int nr) {
-            mark(B200JK_DF_STAGE_J_RHO);
-            for (int q = 0; q < nr; q += 32768 * DFJ_R) {
-                const int m = std::min(32768 * DFJ_R, nr - q);
-                dfj_rho_kernel<<<dim3(nseg, (m + DFJ_R - 1) / DFJ_R, n_dm), 256, 0, st>>>(src, d->d_dmtril, d->d_rho + r0, ld, q, q + m, naux, seglen, ld);
-                launches++;
-            }
-            mark(B200JK_DF_STAGE_J_ACC);
-            const unsigned ncb = (unsigned)((ld + 255) / 256);
-            unsigned gy = (unsigned)std::max<long>(1, std::min<long>(nr / 64, (6L * device_sm_count() * 8 + ncb - 1) / ncb));
-            dfj_acc_kernel<<<dim3(ncb, gy), 256, 0, st>>>(src, d->d_rho + r0, d->d_vjtril, ld, 0, nr, naux, n_dm, ld);
-            launches++;
-            mark(-1);
-            CK(cudaGetLastError());
-        };
-#else
-        auto j_rows = [&](const double* src, int, int nr) {
-            for (int s = 0; s < n_dm; s++)
-                for (int r = 0; r < nr; r++) {
-                    double acc = 0;
-                    for (long t = 0; t < ld; t++) acc += src[(size_t)r * ld + t] * d->d_dmtril[(size_t)s * ld + t];
-                    for (long t = 0; t < ld; t++) d->d_vjtril[(size_t)s * ld + t] += acc * src[(size_t)r * ld + t];
-                }
-        };
-#endif
-        if (vj) {
-            DmTrilFn tf{d->d_dm, d->d_dmtril, nao, ld, d->d_pk_of};     // pair screening: the kept columns only
-            launch_1d((long)n_dm * ld, tf, st); launches++;
-            dev_zero(d->d_vjtril, (size_t)n_dm * ld * 8, st);
-#ifndef B200JK_EMULATE
-            dev_zero(d->d_rho, (size_t)n_dm * naux * 8, st);
-#endif
-            // two streaming passes over the device rows (rho, then J): 2 launches, both HBM-bound
-            (void)rb;
-            if (!streamed || r_dev > r_lo) j_rows(d->d_cderi + (size_t)r_lo * ld, r_lo, r_dev - r_lo);
-            if (!streamed) finish_j();
-        }
-        const bool use_occ = (occ != nullptr && nocc > 0);
-        const int ncol = use_occ ? nocc : nao;
-#ifndef B200JK_EMULATE
-        // tensor-core engine (k_mode 1): the occupied-orbital algorithm when the density carries its orbitals
-        // (pyscf/df/df_jk.py:339-357), else the general-density algorithm (df_jk.py:382-408) with the density itself as
-        // the right factor: Y[nu,(P,k)] = sum_mu A_P[nu,mu] D[mu,k], K[i,l] = sum_(P,k) Y[i,(P,k)] A_P[l,k] — the same two
-        // int8-slice GEMM stages, no cuBLAS
-        const bool tc = d->k_mode == 1;
-        const bool k_sym = use_occ || hermi == 1;   // the result is symmetric: compute the upper triangle, mirror at the end
-#endif
-        std::function<void(const double*, int, int)> k_block;   // K of the rows [r0, r0 + nr) at src (row r0 first)
+        if (vj) j_prepare(c);
+        if (vk) k_prepare(c, occ, r_hi);
+        // the rows: J in two passes over all device rows, then K in blocks; host rows block by block.  With every row in HBM, J
+        // is finished before K starts.
+        const bool resident = d->rows.dev_end(r_lo, r_hi) == r_hi;
+        const int hb = d->kb_max > 0 ? std::min(d->rows.stage_rows, d->kb_max) : d->rows.stage_rows;
+        d->rows.walk(d->d_cderi, r_lo, r_hi, hb, true, st, [&](const double* src, int r0, int nr) {
+            if (vj) j_rows(c, src, r0, nr);
+            if (vj && resident) finish_j(c, vj);
+            if (vk) k_rows(c, src, r0, nr);
+        });
+        if (vj && !resident) finish_j(c, vj);
         if (vk) {
-            if ((size_t)kb > d->ws_rows || (size_t)ncol > d->ws_nocc || (size_t)n_dm > d->ws_occ_ndm) {
-                dev_free(d->d_A); dev_free(d->d_Y); dev_free(d->d_occ);
-                d->d_A = (double*)dev_alloc((size_t)kb * nao * ((nao + 15) & ~15) * 8);   // rows of nao columns padded to 16 (general-density G operand)
-                d->d_Y = (d->k_mode == 1) ? nullptr : (double*)dev_alloc((size_t)kb * ncol * nao * 8);   // FP64 engine only
-                d->d_occ = (double*)dev_alloc((size_t)n_dm * nao * ncol * 8);
-                d->ws_rows = kb; d->ws_nocc = ncol; d->ws_occ_ndm = n_dm;
-            }
-            if (use_occ) {
-                if (!on_device) h2d(d->d_occ, occ, (size_t)n_dm * nao * nocc * 8, st);
-                else {
-#ifndef B200JK_EMULATE
-                    CK(cudaMemcpyAsync(d->d_occ, occ, (size_t)n_dm * nao * nocc * 8, cudaMemcpyDeviceToDevice, st));
-#endif
-                }
-            }
-            dev_zero(d->d_vk, (size_t)n_dm * n2 * 8, st);
-#ifndef B200JK_EMULATE
-            if (tc) {
-                // stage 2 in one K range: pairs(<=ns) * K * 64*64 <= 2^31 - 1 (gemm_ar_acc splits K further where this does not
-                // hold; gemm_ar rejects a stage 1 whose nao breaks the bound)
-                int kmax = (int)(((1L << 31) - 1) / (4096L * d->k_slices));
-                kb = std::max(1, std::min(kb, kmax / ((ncol + 15) & ~15)));   // stage 2 contracts over (P, i) with i padded to 16
-                if ((size_t)kb * ncol * nao > d->y2_cap) { dev_free(d->d_Y2); d->y2_cap = (size_t)kb * ncol * nao; d->d_Y2 = (double*)dev_alloc(d->y2_cap * 8); }
-                if ((size_t)ncol * nao > d->occT_cap) { dev_free(d->d_occT); d->occT_cap = (size_t)ncol * nao; d->d_occT = (double*)dev_alloc(d->occT_cap * 8); }
-                if (!d->d_rowexp) {
-                    d->d_rowexp = (int*)dev_alloc((size_t)std::max(d->nrow, 1) * nao * 4);
-                    d->d_rownorm2 = (float*)dev_alloc((size_t)std::max(d->nrow, 1) * nao * 4);
-                    d->d_cmax2 = (double*)dev_alloc(8);
-                    if (d->n_dev == d->nrow || d->n_dev > 0)     // host rows: per staged block, every call
-                        i8g::packed_rowexp(d->d_cderi, ld, nao, d->n_dev, d->d_rowexp, d->d_rownorm2, st, col_of);
-                }
-            }
-#endif
-#ifndef B200JK_EMULATE
-            if (tc && !(d->sa_decided && d->sa_ns == d->k_slices && d->sa_lo == r_lo && d->sa_hi == r_hi)) {
-                // keep the slices of as many packed rows as fit (7 B per unpacked element): everything when the tensor is small or
-                // sharded over enough GPUs; otherwise a leading part, the rest being re-cut block by block every call
-                size_t freeb = 0, totb = 0;
-                CK(cudaMemGetInfo(&freeb, &totb));
-                freeb += d->SA.cap;                                   // an earlier stack of this handle is reused
-                const size_t kp = ((size_t)nao + 127) / 128 * 128;
-                const size_t per_row = (size_t)d->k_slices * nao * kp;    // bytes of slices per packed row
-                const size_t reserve = (size_t)(kb + 1) * per_row + (12UL << 30);   // the per-block stack + workspaces allocated later
-                const long nloc = r_dev - r_lo;                       // only rows in HBM can be resident
-                long np = 0;
-                if (freeb * 0.85 > (double)reserve) np = (long)((freeb * 0.85 - (double)reserve) / (double)per_row);
-                if (np >= nloc) np = nloc;
-                else if (np < nloc / 10) np = 0;                      // not worth a second code path
-                if (d->np_max >= 0) np = std::min(np, (long)d->np_max);
-                while (np > 0 && (size_t)np * nao >= (1UL << 31) - 256) np--;   // row index of the stack is an int
-                d->sa_np = (int)np;
-                if (np > 0) {
-                    const size_t rows_p = (size_t)np * nao, rp = ((rows_p + 255) / 256) * 256;
-                    d->SA.alloc((int)rows_p, nao, d->k_slices);
-                    CK(cudaMemsetAsync(d->SA.q, 0, (size_t)d->k_slices * rp * kp, st));
-                    CK(cudaMemsetAsync(d->SA.E, 0, rp * 4, st));
-                    i8g::split_packed_into(d->SA, 0, d->d_cderi + (size_t)r_lo * ld, ld, nao, (int)np, d->d_rowexp + (size_t)r_lo * nao, st, col_of);
-                }
-                d->sa_decided = true; d->sa_ns = d->k_slices; d->sa_lo = r_lo; d->sa_hi = r_hi;
-            }
-#endif
-            k_block = [&](const double* src, int r0, int nr) {
-#ifndef B200JK_EMULATE
-                const bool blk_resident = tc && (r0 - r_lo + nr <= d->sa_np);
-                if (tc) {
-                    if (!blk_resident) {    // slices of this block straight from the packed rows
-                        mark(B200JK_DF_STAGE_K_SLICE);
-                        i8g::split_packed(d->SAt, src, ld, nao, nr, d->d_rowexp + (size_t)r0 * nao, d->k_slices, st, col_of);
-                        mark(-1);
-                        launches++;
-                    }
-                    if (!use_occ) {             // general density: the block once more as nao long rows G[l][(P,k)] = A_P[l][k]
-                        mark(B200JK_DF_STAGE_K_SLICE);
-                        // same (P, k) column layout as Y: k padded to 16 when stage 1 cuts the slices of Y itself
-                        static const bool fuse_y_g = getenv("B200JK_NO_YFUSE") == nullptr;
-                        const int gcol = fuse_y_g ? ((nao + 15) & ~15) : nao;
-                        UnpackLongFn ul{src, d->d_A, nao, ld, 0, (long)nr * gcol, gcol, col_of};
-                        launch_1d((long)nao * nr * gcol, ul, st);
-                        i8g::split_rows(d->SG, d->d_A, (long)nr * gcol, nao, nr * gcol, d->k_slices, st);
-                        mark(-1);
-                        launches += 2;
-                    }
-                } else {
-                    UnpackFn up{src, d->d_A, nao, ld, 0, col_of};
-                    launch_1d((long)nr * n2, up, st); launches++;
-                }
-#else
-                UnpackFn up{src, d->d_A, nao, ld, 0, col_of};
-                launch_1d((long)nr * n2, up, st); launches++;
-#endif
-                for (int s = 0; s < n_dm; s++) {
-#ifndef B200JK_EMULATE
-                    const double one = 1.0, zero = 0.0;
-                    if (tc) {
-                        // tensor-core path: Y2[nu][(P,i)] = sum_mu A_P[nu,mu] Ct[i,mu] ; K += Y2 Y2^T (upper triangle)
-                        if (r0 == r_lo || n_dm > 1) {
-                            // right factor of stage 1 as rows [ncol][nao]: C~^T, or D^T for the general-density algorithm
-                            TransposeFn tr{use_occ ? d->d_occ + (size_t)s * nao * nocc : d->d_dm + (size_t)s * n2, d->d_occT, nao, ncol};
-                            launch_1d((long)nao * ncol, tr, st);
-                            i8g::split_rows(d->SC, d->d_occT, nao, ncol, nao, d->k_slices, st); launches += 2;
-                            i8g::colnorm_max(d->d_occT, nao, ncol, nao, d->d_cmax2, st);
-                        }
-                        static const bool prof = getenv("B200JK_DF_PROFILE") != nullptr;
-                        static double tacc[5];
-                        auto tick = [&](int i) {
-                            if (!prof) return;
-                            static std::chrono::steady_clock::time_point last;
-                            CK(cudaStreamSynchronize(st));
-                            auto now = std::chrono::steady_clock::now();
-                            if (i >= 0) tacc[i] += std::chrono::duration<double, std::milli>(now - last).count();
-                            last = now;
-                        };
-                        tick(-1);
-                        tick(0);
-                        mark(B200JK_DF_STAGE_K_GEMM1);
-                        static const bool fuse_y = getenv("B200JK_NO_YFUSE") == nullptr;
-                        if (fuse_y) {
-                            // stage 1 cuts the int8 slices of Y itself: the row exponents are bounded BEFORE the GEMM
-                            // (||A_P[nu,:]||_2 max_i ||C~_i||_2), fp64 Y is never written
-                            const int ncolp = (ncol + 15) & ~15;
-                            i8g::y_prepare(d->SY, nao, nr, ncolp, d->k_slices, d->d_rownorm2 + (size_t)r0 * nao, d->d_cmax2, st);
-                            i8g::gemm_ar(blk_resident ? d->SA : d->SAt, blk_resident ? (r0 - r_lo) * nao : 0, nr * nao, d->SC, nullptr, 0, nao, st,
-                                         nullptr, &d->SY, ncolp);
-                            tick(1);
-                            mark(B200JK_DF_STAGE_K_SLICE);
-                        } else {
-                        // stage 1 leaves the row maxima of Y behind (GemmParams::rowmax): the slicing of Y is one pass
-                        const bool premax = (long)nr * ncol >= 8192;
-                        if (premax) i8g::split_rows_prepare(d->SY, nao, nr * ncol, d->k_slices, st);
-                        i8g::gemm_ar(blk_resident ? d->SA : d->SAt, blk_resident ? (r0 - r_lo) * nao : 0, nr * nao, d->SC, d->d_Y2, (long)nr * ncol, nao, st,
-                                     premax ? d->SY.maxbits : nullptr);
-                        tick(1);
-                        mark(B200JK_DF_STAGE_K_SLICE);
-                        if (premax) i8g::split_rows_premax(d->SY, d->d_Y2, (long)nr * ncol, nao, nr * ncol, d->k_slices, st);
-                        else i8g::split_rows(d->SY, d->d_Y2, (long)nr * ncol, nao, nr * ncol, d->k_slices, st);
-                        }
-                        tick(2);
-                        mark(B200JK_DF_STAGE_K_GEMM2);
-                        // K += Y Y^T (orbitals) or Y G^T (general density; only its upper triangle when D, hence K, is symmetric)
-                        i8g::gemm_ar_acc(d->SY, use_occ ? d->SY : d->SG, d->d_vk + (size_t)s * n2, nao, k_sym, st);
-                        mark(-1);
-                        tick(3);
-                        if (prof && r0 + kb >= r_hi) {
-                            fprintf(stderr, "[df-k profile] zeroY2 %.2f ms, gemm1 %.2f ms, splitY %.2f ms, gemm2 %.2f ms (sum over blocks, kb=%d)\n",
-                                    tacc[0], tacc[1], tacc[2], tacc[3], kb);
-                            for (double& t : tacc) t = 0;
-                        }
-                        launches += 3;
-                        continue;
-                    }
-                    if (use_occ) {
-                        // Y_P (col-major [nao, nocc]) = A_P * Ctilde ; buffers: occ row-major [nao,nocc] == col-major [nocc,nao]
-                        CKB(cublasDgemmStridedBatched(d->cublas, CUBLAS_OP_N, CUBLAS_OP_T, nao, nocc, nao, &one, d->d_A, nao, n2,
-                                                      d->d_occ + (size_t)s * nao * nocc, nocc, 0, &zero, d->d_Y, nao,
-                                                      (long long)nao * nocc, nr));
-                        // K += Z Z^T, Z = [nao, nr*nocc]
-                        CKB(cublasDgemm(d->cublas, CUBLAS_OP_N, CUBLAS_OP_T, nao, nao, nr * nocc, &one, d->d_Y, nao, d->d_Y, nao, &one,
-                                        d->d_vk + (size_t)s * n2, nao));
-                    } else {
-                        // general dm: T_P = A_P * Dbuf (col-major view), K += sum_P T_P * A_P
-                        CKB(cublasDgemmStridedBatched(d->cublas, CUBLAS_OP_N, CUBLAS_OP_N, nao, nao, nao, &one, d->d_A, nao, n2,
-                                                      d->d_dm + (size_t)s * n2, nao, 0, &zero, d->d_Y, nao, n2, nr));
-                        CKB(cublasDgemm(d->cublas, CUBLAS_OP_N, CUBLAS_OP_T, nao, nao, nr * nao, &one, d->d_Y, nao, d->d_A, nao, &one,
-                                        d->d_vk + (size_t)s * n2, nao));
-                    }
-                    launches += 2;
-#else
-                    double* K = d->d_vk + (size_t)s * n2;
-                    if (use_occ) {
-                        // occupied-orbital path (tests only): Y_P = A_P C~ ; K += Y_P Y_P^T — the algebra of the tensor-core engine,
-                        // so that the host-side handling of mo_coeff / mo_occ is exercised on the CPU as well
-                        const double* Cm = d->d_occ + (size_t)s * nao * nocc;     // [nao][nocc]
-                        std::vector<double> Y((size_t)nao * nocc);
-                        for (int r = 0; r < nr; r++) {
-                            const double* A = d->d_A + (size_t)r * n2;
-                            for (int i = 0; i < nao; i++)
-                                for (int o = 0; o < nocc; o++) {
-                                    double acc = 0;
-                                    for (int j = 0; j < nao; j++) acc += A[(size_t)i * nao + j] * Cm[(size_t)j * nocc + o];
-                                    Y[(size_t)i * nocc + o] = acc;
-                                }
-                            for (int i = 0; i < nao; i++)
-                                for (int l = 0; l < nao; l++) {
-                                    double acc = 0;
-                                    for (int o = 0; o < nocc; o++) acc += Y[(size_t)i * nocc + o] * Y[(size_t)l * nocc + o];
-                                    K[(size_t)i * nao + l] += acc;
-                                }
-                        }
-                        continue;
-                    }
-                    // K[i,l] += sum_P sum_jk A_P[i,j] D[j,k] A_P[k,l]   (tests only, O(N^4))
-                    const double* D = d->d_dm + (size_t)s * n2;
-                    std::vector<double> T(n2);
-                    for (int r = 0; r < nr; r++) {
-                        const double* A = d->d_A + (size_t)r * n2;
-                        for (int i = 0; i < nao; i++)
-                            for (int k = 0; k < nao; k++) {
-                                double acc = 0;
-                                for (int j = 0; j < nao; j++) acc += A[(size_t)i * nao + j] * D[(size_t)j * nao + k];
-                                T[(size_t)i * nao + k] = acc;
-                            }
-                        for (int i = 0; i < nao; i++)
-                            for (int l = 0; l < nao; l++) {
-                                double acc = 0;
-                                for (int k = 0; k < nao; k++) acc += T[(size_t)i * nao + k] * A[(size_t)k * nao + l];
-                                K[(size_t)i * nao + l] += acc;
-                            }
-                    }
-#endif
-                }
-            };
-            for (int r0 = r_lo; r0 < r_dev; r0 += kb) k_block(d->d_cderi + (size_t)r0 * ld, r0, std::min(kb, r_dev - r0));
-        }
-        if (streamed) {
-            for (int b = 0; b < nblk; b++) {
-                int r0, nr;
-                blk_rows(b, r0, nr);
-                const double* src = d->d_stage[b & 1];
-#ifndef B200JK_EMULATE
-                CK(cudaEventRecord(d->sx_ev[4 * b + 2], st));
-                CK(cudaStreamWaitEvent(st, d->sx_ev[4 * b + 1], 0));
-                CK(cudaEventRecord(d->sx_ev[4 * b + 3], st));
-#endif
-                if (vj) j_rows(src, r0, nr);
-                if (vk) {
-#ifndef B200JK_EMULATE
-                    if (tc) { i8g::packed_rowexp(src, ld, nao, nr, d->d_rowexp + (size_t)r0 * nao, d->d_rownorm2 + (size_t)r0 * nao, st, col_of); launches++; }
-#endif
-                    for (int q = 0; q < nr; q += kb) k_block(src + (size_t)q * ld, r0 + q, std::min(kb, nr - q));
-                }
-#ifndef B200JK_EMULATE
-                CK(cudaEventRecord(d->ev_free[b & 1], st));
-#endif
-                if (b + 2 < nblk) issue_copy(b + 2);
-                d->stream_bytes += (int64_t)nr * ld * 8;
-            }
-            if (vj) finish_j();
-        }
-        if (vk) {
-#ifndef B200JK_EMULATE
-            if (tc && k_sym) { MirrorUpperFn mf{d->d_vk, nao}; for (int s = 0; s < n_dm; s++) { mf.a = d->d_vk + (size_t)s * n2; launch_1d(n2, mf, st); launches++; } }
-#endif
-            if (!on_device) d2h(vk, d->d_vk, (size_t)n_dm * n2 * 8, st);
-            else {
-#ifndef B200JK_EMULATE
-                CK(cudaMemcpyAsync(vk, d->d_vk, (size_t)n_dm * n2 * 8, cudaMemcpyDeviceToDevice, st));
-#endif
-            }
+            if (c.tc && c.k_sym)
+                for (int s = 0; s < n_dm; s++) { MirrorUpperFn mf{d->d_vk + (size_t)s * c.n2, nao}; launch_1d(c.n2, mf, st); c.launches++; }
+            copy_out(vk, d->d_vk, (size_t)n_dm * c.n2 * 8, on_device, st);
         }
 #ifndef B200JK_EMULATE
         CK(cudaEventRecord(h->ev1, st));
@@ -1646,24 +1715,11 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
         float ms = 0;
         CK(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
         h->stats.ms_kernels = ms;
-        for (int i = 0; i < B200JK_DF_NSTAGE; i++) { d->stage_ms[i] = 0; d->stage_n[i] = 0; }
-        for (size_t i = 0; i + 1 < d->tm_used; i++) {
-            int tag = d->tm_tag[i];
-            if (tag < 0) continue;
-            float t = 0;
-            CK(cudaEventElapsedTime(&t, d->tm_ev[i], d->tm_ev[i + 1]));
-            d->stage_ms[tag] += t; d->stage_n[tag]++;
-        }
-        for (int b = 0; b < nblk; b++) {
-            float tc_ = 0, tw = 0;
-            CK(cudaEventElapsedTime(&tc_, d->sx_ev[4 * b], d->sx_ev[4 * b + 1]));
-            CK(cudaEventElapsedTime(&tw, d->sx_ev[4 * b + 2], d->sx_ev[4 * b + 3]));
-            d->stream_copy_ms += tc_; d->stream_exposed_ms += tw;
-        }
+        d->timer.read(d->stage_ms, d->stage_n);
+        d->rows.read_times();
 #endif
-        auto t1 = std::chrono::steady_clock::now();
-        h->stats.ms_total = std::chrono::duration<double, std::milli>(t1 - t0).count();
-        h->stats.kernel_launches = launches;
+        h->stats.ms_total = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        h->stats.kernel_launches = c.launches;
     } catch (std::exception& e) { set_err(h, e.what()); return 2; }
     return 0;
 }
@@ -1743,14 +1799,14 @@ extern "C" int b200jk_df_pair_stats(b200jk_handle h, int64_t* ncol, int64_t* npa
 extern "C" int b200jk_df_row_split(b200jk_handle h, int* n_dev, int* n_host)
 {
     if (!h || !h->df || !n_dev || !n_host) { set_err(h, "call b200jk_df_build first"); return 1; }
-    *n_dev = h->df->n_dev; *n_host = h->df->nrow - h->df->n_dev;
+    *n_dev = h->df->rows.n_dev; *n_host = h->df->nrow - h->df->rows.n_dev;
     return 0;
 }
 
 extern "C" int b200jk_df_stream_stats(b200jk_handle h, int64_t* bytes, double* copy_ms, double* exposed_ms)
 {
     if (!h || !h->df || !bytes || !copy_ms || !exposed_ms) { set_err(h, "call b200jk_df_build first"); return 1; }
-    *bytes = h->df->stream_bytes; *copy_ms = h->df->stream_copy_ms; *exposed_ms = h->df->stream_exposed_ms;
+    *bytes = h->df->rows.bytes; *copy_ms = h->df->rows.copy_ms; *exposed_ms = h->df->rows.exposed_ms;
     return 0;
 }
 

@@ -303,10 +303,7 @@ static void band_pipeline(DFState* d, stream_t st, int nb, size_t cap, FC comput
     double* dbuf[2] = {(double*)dev_alloc(cap), nb > 1 ? (double*)dev_alloc(cap) : nullptr};
     size_t bytes[2] = {0, 0};
 #ifndef B200JK_EMULATE
-    if (!d->cp_stream) {
-        CK(cudaStreamCreateWithFlags(&d->cp_stream, cudaStreamNonBlocking));
-        for (cudaEvent_t& e : d->ev_free) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    }
+    const cudaStream_t cs = d->rows.copy_stream();
     if (d->pin_cap < cap) {
         for (double*& p : d->h_pin) { if (p) CK(cudaFreeHost(p)); p = nullptr; }
         d->pin_cap = 0;
@@ -332,9 +329,9 @@ static void band_pipeline(DFState* d, stream_t st, int nb, size_t cap, FC comput
             bytes[s] = compute(b, dbuf[s]);
             CK(cudaEventRecord(ev[5 + 2 * s], st));
             CK(cudaEventRecord(ev[s], st));
-            CK(cudaStreamWaitEvent(d->cp_stream, ev[s], 0));
-            CK(cudaMemcpyAsync(hbuf[s], dbuf[s], bytes[s], cudaMemcpyDeviceToHost, d->cp_stream));
-            CK(cudaEventRecord(ev[2 + s], d->cp_stream));
+            CK(cudaStreamWaitEvent(cs, ev[s], 0));
+            CK(cudaMemcpyAsync(hbuf[s], dbuf[s], bytes[s], cudaMemcpyDeviceToHost, cs));
+            CK(cudaEventRecord(ev[2 + s], cs));
             if (b + 1 < nb) CK(cudaStreamWaitEvent(st, ev[2 + (s ^ 1)], 0));   // the next band overwrites the other buffer
         }
         for (int b = std::max(0, nb - 2); b < nb; b++) drain(b);
@@ -415,7 +412,6 @@ extern "C" int b200jk_df_ao2mo(b200jk_handle h, const double* c1, int n1, const 
         const long nij = pr[0].nij, nkl = pr[npr - 1].nij;
         // row blocks of stage 1: Y of a block at most 512 MiB; host rows go through the staging buffers
         int rb = (int)std::max<long>(1, std::min<long>(std::max(nrow, 1), (512L << 20) / ((long)nao * na_max * 8)));
-        const int hb = nrow > d->n_dev ? std::min(rb, d->stage_rows) : 0;
         const long band = ao2mo_band_rows(d, nij, nkl * 8);
         ao2mo_check_fit(8.0 * ((double)nrow * (nij + (same ? 0 : nkl)) + (double)rb * nao * na_max + 2.0 * band * nkl),
                         "the half-transformed integrals L[naux, nij] (and L[naux, nkl]) with their work buffers");
@@ -453,49 +449,9 @@ extern "C" int b200jk_df_ao2mo(b200jk_handle h, const double* c1, int n1, const 
                 }
                 mark();
             };
-            for (int r0 = 0; r0 < d->n_dev; r0 += rb) half(d->d_cderi + (size_t)r0 * ld, r0, std::min(rb, d->n_dev - r0));
-            if (hb > 0) {
-                const int nblk = (nrow - d->n_dev + hb - 1) / hb;
-#ifndef B200JK_EMULATE
-                if (!d->cp_stream) {
-                    CK(cudaStreamCreateWithFlags(&d->cp_stream, cudaStreamNonBlocking));
-                    for (cudaEvent_t& e : d->ev_free) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-                }
-                cudaEvent_t copied[2], start;
-                for (cudaEvent_t& e : copied) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-                CK(cudaEventCreateWithFlags(&start, cudaEventDisableTiming));
-                CK(cudaEventRecord(start, st));
-                CK(cudaStreamWaitEvent(d->cp_stream, start, 0));     // the coefficient uploads are ordered before the copies
-#endif
-                auto issue = [&](int b) {
-                    const int a = d->n_dev + b * hb, nr = std::min(hb, nrow - a);
-#ifndef B200JK_EMULATE
-                    if (b >= 2) CK(cudaStreamWaitEvent(d->cp_stream, d->ev_free[b & 1], 0));
-                    CK(cudaMemcpyAsync(d->d_stage[b & 1], d->h_cderi + (size_t)(a - d->n_dev) * ld, (size_t)nr * ld * 8,
-                                       cudaMemcpyHostToDevice, d->cp_stream));
-                    CK(cudaEventRecord(copied[b & 1], d->cp_stream));
-#else
-                    memcpy(d->d_stage[b & 1], d->h_cderi + (size_t)(a - d->n_dev) * ld, (size_t)nr * ld * 8);
-#endif
-                };
-                for (int b = 0; b < std::min(nblk, 2); b++) issue(b);
-                for (int b = 0; b < nblk; b++) {
-                    const int a = d->n_dev + b * hb, nr = std::min(hb, nrow - a);
-#ifndef B200JK_EMULATE
-                    CK(cudaStreamWaitEvent(st, copied[b & 1], 0));
-#endif
-                    half(d->d_stage[b & 1], a, nr);
-#ifndef B200JK_EMULATE
-                    CK(cudaEventRecord(d->ev_free[b & 1], st));
-#endif
-                    if (b + 2 < nblk) issue(b + 2);
-                }
-#ifndef B200JK_EMULATE
-                CK(cudaStreamSynchronize(st));
-                for (cudaEvent_t e : copied) cudaEventDestroy(e);
-                cudaEventDestroy(start);
-#endif
-            }
+            d->rows.walk(d->d_cderi, 0, nrow, std::min(rb, d->rows.stage_rows), false, st, [&](const double* src, int r0, int nr) {
+                for (int q = 0; q < nr; q += rb) half(src + (size_t)q * ld, r0 + q, std::min(rb, nr - q));
+            });
 #ifndef B200JK_EMULATE
             CK(cudaStreamSynchronize(st));
             for (size_t i = 0; i + 1 < tev.size(); i += 2) { float t = 0; CK(cudaEventElapsedTime(&t, tev[i], tev[i + 1])); ms1 += t; }
@@ -537,7 +493,7 @@ extern "C" int b200jk_df_get_ao_eri(b200jk_handle h, double* out)
         auto t_start = std::chrono::steady_clock::now();
         const long npair = d->npair, ld = d->ncol;
         const int* col_of = d->d_col_of;
-        const int nrow = d->nrow, n_dev = d->n_dev;
+        const int nrow = d->nrow, n_dev = d->rows.n_dev;
 #ifndef B200JK_EMULATE
         CK(cudaSetDevice(h->device));
         cudaStream_t st = h->stream;
@@ -564,10 +520,10 @@ extern "C" int b200jk_df_get_ao_eri(b200jk_handle h, double* out)
             };
             part(d->d_cderi, n_dev, 0);
             // host rows (a tensor larger than the device): staged block by block and added
-            for (int a = n_dev; a < nrow; a += d->stage_rows) {
-                const int nr = std::min(d->stage_rows, nrow - a);
-                h2d(d->d_stage[0], d->h_cderi + (size_t)(a - n_dev) * ld, (size_t)nr * ld * 8, st);
-                part(d->d_stage[0], nr, 1);
+            for (int a = n_dev; a < nrow; a += d->rows.stage_rows) {
+                const int nr = std::min(d->rows.stage_rows, nrow - a);
+                h2d(d->rows.d_stage[0], d->rows.host_row(a), (size_t)nr * ld * 8, st);
+                part(d->rows.d_stage[0], nr, 1);
             }
             return (size_t)(r1 * (r1 + 1) / 2 - r0 * (r0 + 1) / 2) * 8;
         }, [&](int b) { return out + rows[b] * (rows[b] + 1) / 2; }, ms2);

@@ -37,6 +37,7 @@ static void* dev_alloc(size_t n) { void* p = nullptr; CK(cudaMalloc(&p, n ? n : 
 static void dev_free(void* p) { if (p) cudaFree(p); }
 static void h2d(void* d, const void* h, size_t n, cudaStream_t s = 0) { CK(cudaMemcpyAsync(d, h, n, cudaMemcpyHostToDevice, s)); }
 static void d2h(void* h, const void* d, size_t n, cudaStream_t s = 0) { CK(cudaMemcpyAsync(h, d, n, cudaMemcpyDeviceToHost, s)); }
+static void d2d(void* dst, const void* src, size_t n, cudaStream_t s = 0) { CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToDevice, s)); }
 static void dev_zero(void* d, size_t n, cudaStream_t s = 0) { CK(cudaMemsetAsync(d, 0, n, s)); }
 static void dev_sync() { CK(cudaDeviceSynchronize()); }
 template <class F>
@@ -60,6 +61,7 @@ static void dev_free(void* p) { free(p); }
 typedef int stream_t;
 static void h2d(void* d, const void* h, size_t n, stream_t = 0) { memcpy(d, h, n); }
 static void d2h(void* h, const void* d, size_t n, stream_t = 0) { memcpy(h, d, n); }
+static void d2d(void* dst, const void* src, size_t n, stream_t = 0) { memcpy(dst, src, n); }
 static void dev_zero(void* d, size_t n, stream_t = 0) { memset(d, 0, n); }
 static void dev_sync() {}
 template <class F>
