@@ -3,7 +3,7 @@
 #pragma once
 #include <cstdlib>
 #include <stdexcept>
-#include "jk_tpq.cuh"
+#include "jk_swq.cuh"
 
 namespace b200jk {
 
@@ -109,6 +109,12 @@ __global__ void __launch_bounds__(TpqCfg<C>::NT) jk_tpq_kernel(const KParams P)
 {
     const int bx = blockIdx.x * P.shard_world + P.shard_rank;
     if (bx < P.nbra) tpq_block<C, SR>(P, bx, blockIdx.y, blockIdx.z);
+}
+template <class C, bool SR>
+__global__ void __launch_bounds__(SwqCfg<C>::NT) jk_swq_kernel(const KParams P)
+{
+    const int bx = blockIdx.x * P.shard_world + P.shard_rank;
+    if (bx < P.nbra) swq_block<C, SR>(P, bx, blockIdx.y, blockIdx.z);
 }
 // Register cap per class: `__launch_bounds__(192, 2)` (<= 168 registers, two resident CTAs per SM) for most block kernels.
 // The exemptions below are an untuned carry-over, chosen by A/B timing on an earlier GPU generation and not re-timed on the
@@ -240,30 +246,52 @@ void launch_one(KParams P, b2_stream_t st)
                     else tpq_block<C, false>(P, bx, by, bz);
                 }
 #endif
-        return;
-    }
-    const int nbx = (P.nbra + P.shard_world - 1) / P.shard_world;
-    P.kchunk = pick_kchunk(nbx, P.nket, Cfg::GC::NSLOT, kets_cap(KCH_MAX));
-    int ny = (P.nket + P.kchunk - 1) / P.kchunk;
+    } else if constexpr (SwqCfg<C>::eligible) {
+        // contracted three-root classes too large for one thread: T lanes per quartet, registers only (jk_swq.cuh)
+        using W = SwqCfg<C>;
+        P.pslice = W::PSLICE;
+        const int nbx = (P.nbra + P.shard_world - 1) / P.shard_world;   // bra pairs of this rank
+        P.kchunk = pick_kchunk(nbx, P.nket, W::NSLOT, kets_cap(W::KCHUNK));
+        int ny = (P.nket + P.kchunk - 1) / P.kchunk;
 #ifndef B200JK_EMULATE
-    size_t smem = sizeof(BlockSmem<C>);
-    dim3 grid(nbx, ny);
-    if (P.omega < 0.0) launch_block_kernel<C, true>(P, grid, Cfg::NT, smem, st);   // erfc operator: two root sets per primitive quartet
-    else launch_block_kernel<C, false>(P, grid, Cfg::NT, smem, st);
+        dim3 grid(nbx, ny, (P.bra_nprim_max + P.pslice - 1) / P.pslice);
+        if (P.omega < 0.0) jk_swq_kernel<C, true><<<grid, W::NT, 0, st>>>(P);   // erfc operator: two root sets
+        else jk_swq_kernel<C, false><<<grid, W::NT, 0, st>>>(P);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) throw std::runtime_error(std::string("jk_swq_kernel launch: ") + cudaGetErrorString(e));
 #else
-    (void)st;
-    BlockSmem<C>* sm = new BlockSmem<C>();
-    for (int bx = P.shard_rank; bx < P.nbra; bx += P.shard_world)
-        for (int by = 0; by < ny; by++) {
-            if (P.omega < 0.0) jk_block<C, true>(P, bx, by, *sm);
-            else jk_block<C, false>(P, bx, by, *sm);
-        }
-    delete sm;
+        (void)st;
+        for (int bx = P.shard_rank; bx < P.nbra; bx += P.shard_world)
+            for (int by = 0; by < ny; by++)
+                for (int bz = 0; bz * P.pslice < P.bra_nprim_max; bz++) {
+                    if (P.omega < 0.0) swq_block<C, true>(P, bx, by, bz);
+                    else swq_block<C, false>(P, bx, by, bz);
+                }
 #endif
+    } else {
+        const int nbx = (P.nbra + P.shard_world - 1) / P.shard_world;
+        P.kchunk = pick_kchunk(nbx, P.nket, Cfg::GC::NSLOT, kets_cap(KCH_MAX));
+        int ny = (P.nket + P.kchunk - 1) / P.kchunk;
+#ifndef B200JK_EMULATE
+        size_t smem = sizeof(BlockSmem<C>);
+        dim3 grid(nbx, ny);
+        if (P.omega < 0.0) launch_block_kernel<C, true>(P, grid, Cfg::NT, smem, st);   // erfc operator: two root sets per primitive quartet
+        else launch_block_kernel<C, false>(P, grid, Cfg::NT, smem, st);
+#else
+        (void)st;
+        BlockSmem<C>* sm = new BlockSmem<C>();
+        for (int bx = P.shard_rank; bx < P.nbra; bx += P.shard_world)
+            for (int by = 0; by < ny; by++) {
+                if (P.omega < 0.0) jk_block<C, true>(P, bx, by, *sm);
+                else jk_block<C, false>(P, bx, by, *sm);
+            }
+        delete sm;
+#endif
+    }
 }
 
 // Launch shape of a class as launch_one launches it (the omega >= 0 entry point), out[B2_LAUNCH_INFO_N]:
-//   [0] family: 0 thread-per-quartet, 1 block     [1] threads per CTA     [2] dynamic shared memory per CTA (bytes)
+//   [0] family: 0 thread-per-quartet, 1 block, 2 sub-warp per quartet     [1] threads per CTA     [2] dynamic shared memory per CTA (bytes)
 //   [3] registers per thread     [4] local memory per thread (bytes; > 0 means spills)
 //   [5] CTAs per SM by the occupancy API under the carve-out set     [6] carve-out set (percent; -1: none)
 //   [7] CTAs per SM that registers and threads alone allow     [8] 1 if launched with bra and ket swapped (use_swapped)
@@ -281,6 +309,11 @@ void info_one(int* out)
         out[0] = 0; out[1] = TpqCfg<C>::NT;
 #ifndef B200JK_EMULATE
         kern = (const void*)jk_tpq_kernel<C, false>;
+#endif
+    } else if constexpr (SwqCfg<C>::eligible) {
+        out[0] = 2; out[1] = SwqCfg<C>::NT;
+#ifndef B200JK_EMULATE
+        kern = (const void*)jk_swq_kernel<C, false>;
 #endif
     } else {
         out[0] = 1; out[1] = Cfg::NT; smem = sizeof(BlockSmem<C>);

@@ -73,7 +73,7 @@ def main():
           % (name, power, min(ms), np.mean(ms), best.sum()))
     print('%-9s %-5s %4s %7s %4s %5s %5s %5s %5s %8s' % ('class', 'fam', 'thr', 'smem', 'reg', 'local', 'carve', 'cta', 'ctaR', 'ms'))
     for k, r in sorted(rows.items(), key=lambda kv: -kv[1]['ms']):
-        print('%-9s %-5s %4d %7d %4d %5d %5d %5d %5d %8.3f%s' % (k, 'block' if r['family'] else 'tpq', r['threads'], r['smem'],
+        print('%-9s %-5s %4d %7d %4d %5d %5d %5d %5d %8.3f%s' % (k, ('tpq', 'block', 'swq')[r['family']], r['threads'], r['smem'],
               r['regs'], r['local'], r['carveout'], r['ctas_sm'], r['ctas_regs'], r['ms'], ' swapped' if r['swapped'] else ''))
     if a.json:
         d = os.path.dirname(os.path.abspath(a.json))
