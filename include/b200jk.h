@@ -28,6 +28,8 @@
  *   b200jk_df_ao2mo          DF.ao2mo = get_mo_eri               pyscf/df/df.py:278-296
  *                            -> _ao2mo.nr_e2 + lib.dot           pyscf/ao2mo/_ao2mo.py:157, pyscf/lib/ao2mo/nr_ao2mo.c:1240
  *   b200jk_df_get_ao_eri     DF.get_eri = get_ao_eri             pyscf/df/df.py:269-276 (+ ao2mo.restore(8))
+ *   b200jk_df_mp2            DFRMP2 / DFUMP2 kernel              pyscf/mp/dfmp2.py:39-121, dfump2.py:38-166
+ *                            -> MP2_contract_d, MP2_OS_contract_d pyscf/lib/mp/mp2.c:89-275
  *   b200jk_get_stats         (no reference equivalent; logger.timer 'vj and vk' pyscf/scf/hf.py:2158)
  *
  * Conventions: all matrices are C-contiguous fp64 in the reference's spherical AO order;
@@ -150,6 +152,17 @@ int b200jk_df_set_ao2mo_tile(b200jk_handle h, int max_rows);
 /* Times of the last b200jk_df_ao2mo / b200jk_df_get_ao_eri (no reference equivalent): ms[0] stage-1 and ms[1] stage-2 device
  * time (CUDA events around the launches), ms[2] host wall time of the whole call including the copies; n <= 3 entries. */
 int b200jk_df_ao2mo_times(b200jk_handle h, double* ms, int n);
+/* DFMP2 / DFUMP2 kernel (pyscf/mp/dfmp2.py:39-121, dfump2.py:38-166): nspin 1 or 2; per spin s occupied / virtual
+ * coefficients c_occ[s] [nao][nocc[s]] / c_vir[s] [nao][nvir[s]] (host, C-contiguous) and orbital energies e_occ[s] / e_vir[s].
+ * e_out[0] = same-spin, e_out[1] = opposite-spin part of the correlation energy (e_corr = e_out[0] + e_out[1]).
+ * t2: NULL, or nspin == 1: t2[0] = [nocc, nocc, nvir, nvir]; nspin == 2: t2[0..2] = aa, ab, bb as dfump2.py:51-54 (aa and bb
+ * antisymmetrized as with t2_ex, mp2.c:158-161).  A spin with no occupied or no virtual orbitals contributes exactly 0.
+ * (ia|jb) is formed pair by pair on the device and never leaves it (df_mp2.cuh); the energies are bit-reproducible.  Fails
+ * with a message when L[naux, nocc nvir] of each spin does not fit next to the tensor; a sharded tensor is refused. */
+int b200jk_df_mp2(b200jk_handle h, int nspin, const double* const* c_occ, const int* nocc, const double* const* c_vir,
+                  const int* nvir, const double* const* e_occ, const double* const* e_vir, double* e_out, double* const* t2);
+/* Times of the last b200jk_df_mp2: ms[0] stage-1, ms[1] stage-2 device ms, ms[2] host wall time of the call; n <= 3. */
+int b200jk_df_mp2_times(b200jk_handle h, double* ms, int n);
 
 /* Schwarz table q_cond[nbas,nbas] in the reference's (contracted, spherical-order) shell indexing. */
 int b200jk_get_q_cond(b200jk_handle h, double* q_cond, int nbas);

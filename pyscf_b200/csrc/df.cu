@@ -6,6 +6,8 @@
 //   b200jk_df_jk    : J = cderi^T (cderi . dmtril) ; K = sum_P (P|.i)(P|.i)^T  <- df_jk.get_jk, pyscf/df/df_jk.py:280-413
 //   b200jk_df_ao2mo, b200jk_df_get_ao_eri : MO / AO integrals from the tensor      <- DF.ao2mo / get_eri, pyscf/df/df.py:269-296
 //                     (df_ao2mo.cuh, FP64 tensor-core GEMMs)
+//   b200jk_df_mp2   : DF-MP2 energies and amplitudes from the tensor            <- DFRMP2 / DFUMP2, pyscf/mp/dfmp2.py:39-121,
+//                     (df_mp2.cuh, the same GEMM core)                              dfump2.py:38-166
 // The tensor stays resident in HBM in the reference's own layout (row P, packed lower triangle mu>=nu).
 #include "host_common.hpp"
 #include "df_classes.cuh"
@@ -329,6 +331,7 @@ struct DFState {
     double ao2mo_ms[3] = {0, 0, 0};
     int ao2mo_tile_rows = -1;
     double* h_pin[2] = {nullptr, nullptr}; size_t pin_cap = 0;   // pinned staging of the output bands, kept between calls
+    double mp2_ms[3] = {0, 0, 0};   // DF-MP2 (df_mp2.cuh): device ms of stage 1 and stage 2, host ms of the last call
 };
 
 namespace {
@@ -1820,3 +1823,4 @@ extern "C" int b200jk_df_set_kmode(b200jk_handle h, int mode, int nslices)
 }
 
 #include "df_ao2mo.cuh"
+#include "df_mp2.cuh"

@@ -294,11 +294,12 @@ static void par_memcpy(void* dst, const void* src, size_t n)
 }
 
 // Bands b = 0..nb-1 of the output: compute(b, dbuf) fills a device buffer on the compute stream and returns its bytes; the copy
-// to a pinned buffer runs on the copy stream while band b + 1 is computed, and the host then moves it to dst(b).  cap: bytes
-// of the largest band.  ms2 accumulates the device time of compute().  The two pinned buffers stay on the handle (h_pin) for
-// the next call: a CASSCF macro iteration calls ao2mo every time, and pinning hundreds of MB costs more than a small transform.
-template <class FC, class FD>
-static void band_pipeline(DFState* d, stream_t st, int nb, size_t cap, FC compute, FD dst, double& ms2)
+// to a pinned buffer runs on the copy stream while band b + 1 is computed, and the host then hands it to sink(b, src, bytes),
+// which moves it into the caller's array.  cap: bytes of the largest band.  ms2 accumulates the device time of compute().  The
+// two pinned buffers stay on the handle (h_pin) for the next call: a CASSCF macro iteration calls ao2mo every time, and pinning
+// hundreds of MB costs more than a small transform.
+template <class FC, class FS>
+static void band_pipeline(DFState* d, stream_t st, int nb, size_t cap, FC compute, FS sink, double& ms2)
 {
     double* dbuf[2] = {(double*)dev_alloc(cap), nb > 1 ? (double*)dev_alloc(cap) : nullptr};
     size_t bytes[2] = {0, 0};
@@ -320,7 +321,7 @@ static void band_pipeline(DFState* d, stream_t st, int nb, size_t cap, FC comput
             float t = 0;
             CK(cudaEventElapsedTime(&t, ev[4 + 2 * s], ev[5 + 2 * s]));
             ms2 += t;
-            par_memcpy(dst(b), hbuf[s], bytes[s]);
+            sink(b, hbuf[s], bytes[s]);
         };
         for (int b = 0; b < nb; b++) {
             const int s = b & 1;
@@ -346,7 +347,7 @@ static void band_pipeline(DFState* d, stream_t st, int nb, size_t cap, FC comput
     (void)d; (void)st; (void)ms2;
     for (int b = 0; b < nb; b++) {
         bytes[b & 1] = compute(b, dbuf[b & 1]);
-        memcpy(dst(b), dbuf[b & 1], bytes[b & 1]);
+        sink(b, dbuf[b & 1], bytes[b & 1]);
     }
 #endif
     dev_free(dbuf[0]); dev_free(dbuf[1]);
@@ -378,6 +379,66 @@ static void ao2mo_check_fit(double need, const char* what)
 #endif
 }
 
+// One coefficient pair of stage 1: host sets c[0] [nao][n[0]] and c[1] [nao][n[1]], their device copies dc, and the output
+// L[P][nij] (s2: i >= j at i(i+1)/2 + j, else i n[1] + j) over the local rows P.
+struct HalfPair { const double* c[2]; int n[2]; int s2; long nij; double* L; double* dc[2]; };
+
+// tensor rows per stage-1 block: Y of a block at most 512 MiB; na_max = largest set contracted first
+static int half_block_rows(int nrow, int nao, int na_max)
+{
+    return (int)std::max<long>(1, std::min<long>(std::max(nrow, 1), (512L << 20) / ((long)nao * na_max * 8)));
+}
+
+// Stage 1 on the compute stream: L of every pair in pr[0, npr) from all local rows (device rows in place, host rows through the
+// staging buffers), in blocks of rb rows through d_Y [rb][nao][na_max].  Returns the device ms of the GEMMs.
+static double half_transform(DFState* d, int nao, stream_t st, HalfPair* pr, int npr, double* d_Y, int rb)
+{
+    const int nrow = d->nrow;
+    const long ld = d->ncol;
+    const int* col_of = d->d_col_of;
+    double ms1 = 0.0;
+#ifndef B200JK_EMULATE
+    std::vector<cudaEvent_t> tev;
+    auto mark = [&]() { cudaEvent_t e; CK(cudaEventCreate(&e)); CK(cudaEventRecord(e, st)); tev.push_back(e); };
+#else
+    auto mark = [&]() {};
+#endif
+    // ---- stage 1 on the rows [r0, r0 + nr) at src
+    auto half = [&](const double* src, int r0, int nr) {
+        mark();
+        for (int q = 0; q < npr; q++) {
+            HalfPair& p = pr[q];
+            const int f = p.n[0] <= p.n[1] ? 0 : 1;     // the smaller set is contracted first
+            const int na = p.n[f], nb_ = p.n[1 - f];
+            ao2mo::Gemm<ao2mo::TriRowsA, ao2mo::RowsB, ao2mo::RowsSt> g1{(long)nr * nao, na, nao, {src, ld, col_of, nao},
+                                                                          {p.dc[f], na}, {d_Y, na}, 0, 0, 0};
+            ao2mo::gemm(g1, st);
+            ao2mo::Gemm<ao2mo::TransA, ao2mo::YColsB, ao2mo::LSt> g2{nb_, (long)nr * na, nao, {p.dc[1 - f], nb_}, {d_Y, nao, na},
+                                                                     {p.L + (size_t)r0 * p.nij, p.nij, na, p.n[1], f == 1, p.s2}, 0, 0, 0};
+            ao2mo::gemm(g2, st);
+        }
+        mark();
+    };
+    try {
+        d->rows.walk(d->d_cderi, 0, nrow, std::min(rb, d->rows.stage_rows), false, st, [&](const double* src, int r0, int nr) {
+            for (int q = 0; q < nr; q += rb) half(src + (size_t)q * ld, r0 + q, std::min(rb, nr - q));
+        });
+#ifndef B200JK_EMULATE
+        CK(cudaStreamSynchronize(st));
+        for (size_t i = 0; i + 1 < tev.size(); i += 2) { float t = 0; CK(cudaEventElapsedTime(&t, tev[i], tev[i + 1])); ms1 += t; }
+#endif
+    } catch (...) {
+#ifndef B200JK_EMULATE
+        for (cudaEvent_t e : tev) cudaEventDestroy(e);
+#endif
+        throw;
+    }
+#ifndef B200JK_EMULATE
+    for (cudaEvent_t e : tev) cudaEventDestroy(e);
+#endif
+    return ms1;
+}
+
 extern "C" int b200jk_df_ao2mo(b200jk_handle h, const double* c1, int n1, const double* c2, int n2, int s2_12, const double* c3,
                                int n3, const double* c4, int n4, int s2_34, double* out)
 {
@@ -392,26 +453,22 @@ extern "C" int b200jk_df_ao2mo(b200jk_handle h, const double* c1, int n1, const 
         if ((s2_12 && n1 != n2) || (s2_34 && n3 != n4)) throw std::runtime_error("an s2 pair needs two sets of equal size");
         auto t_start = std::chrono::steady_clock::now();
         const int nao = h->nsph, nrow = d->nrow;
-        const long ld = d->ncol;
-        const int* col_of = d->d_col_of;
 #ifndef B200JK_EMULATE
         CK(cudaSetDevice(h->device));
         cudaStream_t st = h->stream;
 #else
         stream_t st = 0;
 #endif
-        struct Pair { const double* c[2]; int n[2]; int s2; long nij; double* L; double* dc[2]; };
-        Pair pr[2] = {{{c1, c2}, {n1, n2}, s2_12, 0, nullptr, {nullptr, nullptr}},
-                      {{c3, c4}, {n3, n4}, s2_34, 0, nullptr, {nullptr, nullptr}}};
+        HalfPair pr[2] = {{{c1, c2}, {n1, n2}, s2_12, 0, nullptr, {nullptr, nullptr}},
+                          {{c3, c4}, {n3, n4}, s2_34, 0, nullptr, {nullptr, nullptr}}};
         const int npr = same ? 1 : 2;
         int na_max = 1;
-        for (Pair& p : pr) {
+        for (HalfPair& p : pr) {
             p.nij = p.s2 ? (long)p.n[0] * (p.n[0] + 1) / 2 : (long)p.n[0] * p.n[1];
             na_max = std::max(na_max, std::min(p.n[0], p.n[1]));
         }
         const long nij = pr[0].nij, nkl = pr[npr - 1].nij;
-        // row blocks of stage 1: Y of a block at most 512 MiB; host rows go through the staging buffers
-        int rb = (int)std::max<long>(1, std::min<long>(std::max(nrow, 1), (512L << 20) / ((long)nao * na_max * 8)));
+        const int rb = half_block_rows(nrow, nao, na_max);
         const long band = ao2mo_band_rows(d, nij, nkl * 8);
         ao2mo_check_fit(8.0 * ((double)nrow * (nij + (same ? 0 : nkl)) + (double)rb * nao * na_max + 2.0 * band * nkl),
                         "the half-transformed integrals L[naux, nij] (and L[naux, nkl]) with their work buffers");
@@ -426,37 +483,8 @@ extern "C" int b200jk_df_ao2mo(b200jk_handle h, const double* c1, int n1, const 
                 }
             }
             double* d_Y = alloc((size_t)rb * nao * na_max);
-            double ms1 = 0.0, ms2 = 0.0;
-#ifndef B200JK_EMULATE
-            std::vector<cudaEvent_t> tev;
-            auto mark = [&]() { cudaEvent_t e; CK(cudaEventCreate(&e)); CK(cudaEventRecord(e, st)); tev.push_back(e); };
-#else
-            auto mark = [&]() {};
-#endif
-            // ---- stage 1 on the rows [r0, r0 + nr) at src
-            auto half = [&](const double* src, int r0, int nr) {
-                mark();
-                for (int q = 0; q < npr; q++) {
-                    Pair& p = pr[q];
-                    const int f = p.n[0] <= p.n[1] ? 0 : 1;     // the smaller set is contracted first
-                    const int na = p.n[f], nb_ = p.n[1 - f];
-                    ao2mo::Gemm<ao2mo::TriRowsA, ao2mo::RowsB, ao2mo::RowsSt> g1{(long)nr * nao, na, nao, {src, ld, col_of, nao},
-                                                                                  {p.dc[f], na}, {d_Y, na}, 0, 0, 0};
-                    ao2mo::gemm(g1, st);
-                    ao2mo::Gemm<ao2mo::TransA, ao2mo::YColsB, ao2mo::LSt> g2{nb_, (long)nr * na, nao, {p.dc[1 - f], nb_}, {d_Y, nao, na},
-                                                                             {p.L + (size_t)r0 * p.nij, p.nij, na, p.n[1], f == 1, p.s2}, 0, 0, 0};
-                    ao2mo::gemm(g2, st);
-                }
-                mark();
-            };
-            d->rows.walk(d->d_cderi, 0, nrow, std::min(rb, d->rows.stage_rows), false, st, [&](const double* src, int r0, int nr) {
-                for (int q = 0; q < nr; q += rb) half(src + (size_t)q * ld, r0 + q, std::min(rb, nr - q));
-            });
-#ifndef B200JK_EMULATE
-            CK(cudaStreamSynchronize(st));
-            for (size_t i = 0; i + 1 < tev.size(); i += 2) { float t = 0; CK(cudaEventElapsedTime(&t, tev[i], tev[i + 1])); ms1 += t; }
-            for (cudaEvent_t e : tev) cudaEventDestroy(e);
-#endif
+            const double ms1 = half_transform(d, nao, st, pr, npr, d_Y, rb);
+            double ms2 = 0.0;
             // ---- stage 2: bands of output rows [r0, r1)
             const double* Lij = pr[0].L;
             const double* Lkl = pr[npr - 1].L;
@@ -468,7 +496,7 @@ extern "C" int b200jk_df_ao2mo(b200jk_handle h, const double* c1, int n1, const 
                 ao2mo::gemm(g, st);
                 if (same) { ao2mo::MirrorBandFn mf{buf, nkl, r0, r1 - r0}; launch_1d((r1 - r0) * (r1 - r0), mf, st); }
                 return (size_t)(r1 - r0) * nkl * 8;
-            }, [&](int b) { return out + (size_t)b * band * nkl; }, ms2);
+            }, [&](int b, const void* src, size_t n) { ao2mo::par_memcpy(out + (size_t)b * band * nkl, src, n); }, ms2);
             d->ao2mo_ms[0] = ms1; d->ao2mo_ms[1] = ms2;
         } catch (...) {
             dev_sync();
@@ -526,7 +554,7 @@ extern "C" int b200jk_df_get_ao_eri(b200jk_handle h, double* out)
                 part(d->rows.d_stage[0], nr, 1);
             }
             return (size_t)(r1 * (r1 + 1) / 2 - r0 * (r0 + 1) / 2) * 8;
-        }, [&](int b) { return out + rows[b] * (rows[b] + 1) / 2; }, ms2);
+        }, [&](int b, const void* src, size_t n) { ao2mo::par_memcpy(out + rows[b] * (rows[b] + 1) / 2, src, n); }, ms2);
         dev_sync();
         d->ao2mo_ms[0] = 0.0; d->ao2mo_ms[1] = ms2;
         d->ao2mo_ms[2] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();

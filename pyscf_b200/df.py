@@ -364,7 +364,7 @@ class DF:
     # ---- MO / AO integrals from the tensor ------------------------------------------------------------
     def ao2mo(self, mo_coeffs, compact=True):
         """(ij|kl) = sum_P L[P, ij] L[P, kl], L[P, ij] = C1[:, i]^T B_P C2[:, j], on the GPU: DF.ao2mo (pyscf/df/df.py:278-296),
-        what mp.MP2, DF-CASSCF and DF-NEVPT2 call on mf.with_df.
+        what DF-CASSCF and DF-NEVPT2 call on mf.with_df (DF-MP2 takes its own route: pyscf_b200.dfmp2).
 
         mo_coeffs: one [nao, n] array (four equal sets) or a sequence of four.  Pair (1,2) is packed s2 (row i(i+1)/2 + j,
         i >= j) when `compact` and its two sets are identical in the sense of iden_coeffs (pyscf/ao2mo/incore.py:239-241),
