@@ -30,6 +30,8 @@
  *   b200jk_df_get_ao_eri     DF.get_eri = get_ao_eri             pyscf/df/df.py:269-276 (+ ao2mo.restore(8))
  *   b200jk_df_mp2            DFRMP2 / DFUMP2 kernel              pyscf/mp/dfmp2.py:39-121, dfump2.py:38-166
  *                            -> MP2_contract_d, MP2_OS_contract_d pyscf/lib/mp/mp2.c:89-275
+ *   b200jk_df_rpa            RPA / URPA kernel                   pyscf/gw/rpa.py:43-130, urpa.py:41-72
+ *                            -> make_dielectric_matrix + log(det(I - Pi)) per frequency  rpa.py:80-84,100-130
  *   b200jk_get_stats         (no reference equivalent; logger.timer 'vj and vk' pyscf/scf/hf.py:2158)
  *
  * Conventions: all matrices are C-contiguous fp64 in the reference's spherical AO order;
@@ -163,6 +165,22 @@ int b200jk_df_mp2(b200jk_handle h, int nspin, const double* const* c_occ, const 
                   const int* nvir, const double* const* e_occ, const double* const* e_vir, double* e_out, double* const* t2);
 /* Times of the last b200jk_df_mp2: ms[0] stage-1, ms[1] stage-2 device ms, ms[2] host wall time of the call; n <= 3. */
 int b200jk_df_mp2_times(b200jk_handle h, double* ms, int n);
+/* Direct-RPA kernel (pyscf/gw/rpa.py:43-130, urpa.py:41-72): nspin 1 (RPA) or 2 (URPA); per spin s occupied / virtual
+ * coefficients c_occ[s] [nao][nocc[s]] / c_vir[s] [nao][nvir[s]] (host, C-contiguous) and e_ov[s] / f_ov[s] [nocc[s] nvir[s]]
+ * (index i nvir + a, as make_e_ov / make_f_ov return them).  For each of the nw frequencies omega[w]:
+ *   Pi(w) = sum_s L_s chi_s(w) L_s^T,  chi_s[ia] = 2 e_ov f_ov / (w^2 + e_ov^2)   (make_dielectric_matrix, rpa.py:100-130)
+ * logdet[w] = log det(I - Pi(w)) from a Cholesky factor and trace[w] = tr Pi(w); e_corr = sum_w weight_w / 2pi (logdet[w] +
+ * trace[w]) (rpa.py:80-84).  diel: NULL, or with nw == 1, Pi(omega[0]) [naux][naux] (full and symmetric, not I - Pi).  A spin
+ * with no occupied or no virtual orbitals contributes nothing.  L_s = C_occ^T B C_vir stays on the device and Pi is formed
+ * there one frequency at a time (df_rpa.cuh); logdet and trace are bit-reproducible up to the factorisation.  Fails with a
+ * message naming omega when I - Pi(omega) is not positive definite, when L and Pi do not fit next to the tensor, and for a
+ * sharded tensor. */
+int b200jk_df_rpa(b200jk_handle h, int nspin, const double* const* c_occ, const int* nocc, const double* const* c_vir,
+                  const int* nvir, const double* const* e_ov, const double* const* f_ov, int nw, const double* omega,
+                  double* logdet, double* trace, double* diel);
+/* Times of the last b200jk_df_rpa: ms[0] stage-1, ms[1] Pi GEMM, ms[2] factorisation device ms (summed over the frequencies),
+ * ms[3] host wall time of the call; n <= 4. */
+int b200jk_df_rpa_times(b200jk_handle h, double* ms, int n);
 
 /* Schwarz table q_cond[nbas,nbas] in the reference's (contracted, spherical-order) shell indexing. */
 int b200jk_get_q_cond(b200jk_handle h, double* q_cond, int nbas);

@@ -8,6 +8,8 @@
 //                     (df_ao2mo.cuh, FP64 tensor-core GEMMs)
 //   b200jk_df_mp2   : DF-MP2 energies and amplitudes from the tensor            <- DFRMP2 / DFUMP2, pyscf/mp/dfmp2.py:39-121,
 //                     (df_mp2.cuh, the same GEMM core)                              dfump2.py:38-166
+//   b200jk_df_rpa   : direct-RPA correlation energy from the tensor             <- RPA / URPA, pyscf/gw/rpa.py:43-130,
+//                     (df_rpa.cuh, the same GEMM core + potrf)                      urpa.py:41-72
 // The tensor stays resident in HBM in the reference's own layout (row P, packed lower triangle mu>=nu).
 #include "host_common.hpp"
 #include "df_classes.cuh"
@@ -332,6 +334,7 @@ struct DFState {
     int ao2mo_tile_rows = -1;
     double* h_pin[2] = {nullptr, nullptr}; size_t pin_cap = 0;   // pinned staging of the output bands, kept between calls
     double mp2_ms[3] = {0, 0, 0};   // DF-MP2 (df_mp2.cuh): device ms of stage 1 and stage 2, host ms of the last call
+    double rpa_ms[4] = {0, 0, 0, 0};   // DF-RPA (df_rpa.cuh): device ms of stage 1, the Pi GEMMs, the factorisations; host ms
 };
 
 namespace {
@@ -1824,3 +1827,4 @@ extern "C" int b200jk_df_set_kmode(b200jk_handle h, int mode, int nslices)
 
 #include "df_ao2mo.cuh"
 #include "df_mp2.cuh"
+#include "df_rpa.cuh"

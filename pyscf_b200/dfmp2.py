@@ -27,20 +27,20 @@ class TaggedFloat(float):
         return x
 
 
-def _check_df(with_df):
+def _check_df(with_df, method='DF-MP2', why='the pair energies are not linear in the local rows'):
+    """nao of a built, unsharded with_df (shared with pyscf_b200.rpa, which passes its own method name and reason)."""
     if with_df.shard is not None:
-        raise NotImplementedError('DF-MP2 on a sharded tensor (DF(shard=...)) is not implemented: the pair energies are not '
-                                  'linear in the local rows')
+        raise NotImplementedError('%s on a sharded tensor (DF(shard=...)) is not implemented: %s' % (method, why))
     with_df.get_naoaux()
     return with_df.nao
 
 
-def _coeff(c, nao, what):
+def _coeff(c, nao, what, method='DF-MP2'):
     a = np.asarray(c)
     if np.iscomplexobj(a):
-        raise NotImplementedError('DF-MP2: complex MO coefficients are not supported')
+        raise NotImplementedError('%s: complex MO coefficients are not supported' % method)
     if a.ndim != 2 or a.shape[0] != nao:
-        raise ValueError('DF-MP2: %s coefficients must be [nao, n] with nao = %d, got shape %s' % (what, nao, a.shape))
+        raise ValueError('%s: %s coefficients must be [nao, n] with nao = %d, got shape %s' % (method, what, nao, a.shape))
     return np.ascontiguousarray(a, dtype=np.float64)
 
 

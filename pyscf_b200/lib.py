@@ -47,7 +47,8 @@ SYMBOLS = ['b200jk_create', 'b200jk_create2', 'b200jk_destroy', 'b200jk_set_scre
            'b200jk_df_set_device_rows', 'b200jk_df_row_split', 'b200jk_df_stream_stats',
            'b200jk_df_set_pair_tol', 'b200jk_df_pair_stats', 'b200jk_rys_test', 'b200jk_df_set_raw_test',
            'b200jk_df_get_metric_test', 'b200jk_get_dm_cond_test', 'b200jk_df_ao2mo', 'b200jk_df_get_ao_eri',
-           'b200jk_df_set_ao2mo_tile', 'b200jk_df_ao2mo_times', 'b200jk_df_mp2', 'b200jk_df_mp2_times']
+           'b200jk_df_set_ao2mo_tile', 'b200jk_df_ao2mo_times', 'b200jk_df_mp2', 'b200jk_df_mp2_times',
+           'b200jk_df_rpa', 'b200jk_df_rpa_times']
 
 
 def load(path=None):
@@ -104,6 +105,9 @@ def load(path=None):
     lib.b200jk_df_mp2.argtypes = [vp, ctypes.c_int, c_double_pp, c_int_p, c_double_pp, c_int_p, c_double_pp, c_double_pp, c_double_p,
                                   c_double_pp]
     lib.b200jk_df_mp2_times.argtypes = [vp, c_double_p, ctypes.c_int]
+    lib.b200jk_df_rpa.argtypes = [vp, ctypes.c_int, c_double_pp, c_int_p, c_double_pp, c_int_p, c_double_pp, c_double_pp, ctypes.c_int,
+                                  c_double_p, c_double_p, c_double_p, c_double_p]
+    lib.b200jk_df_rpa_times.argtypes = [vp, c_double_p, ctypes.c_int]
     lib.b200jk_df_local_rows.argtypes = [vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]
     lib.b200jk_set_shard.argtypes = [vp, ctypes.c_int, ctypes.c_int]
     lib.b200jk_df_jk_device.argtypes = [vp, vp, ctypes.c_int, ctypes.c_int, vp, ctypes.c_int, ctypes.c_int, vp, vp]
