@@ -11,6 +11,9 @@
 //   b200jk_df_rpa   : direct-RPA correlation energy from the tensor             <- RPA / URPA, pyscf/gw/rpa.py:43-130,
 //                     (df_rpa.cuh, the same GEMM core + potrf)                      urpa.py:41-72
 // The tensor stays resident in HBM in the reference's own layout (row P, packed lower triangle mu>=nu).
+// The four MO consumers of the tensor (ao2mo, get_ao_eri, DF-MP2, DF-RPA) share one call harness (MoCall), one stage 1
+// (half_transform) and one CTA k loop on the FP64 GEMM core (ao2mo::k_loop); all of them, get_ao_eri included, visit the host
+// rows through RowSplit::walk.
 #include "host_common.hpp"
 #include "df_classes.cuh"
 
@@ -239,29 +242,37 @@ struct RowSplit {
 #endif
 };
 
+// Per-stage device timers: mark(tag) ... mark(-1) brackets one stage with CUDA events on the stream, without host
+// synchronisation; read() adds the brackets of each tag in [0, nstage) up into ms (and counts them into n unless it is null)
+// once the stream is synchronised.  The emulation has no device time: read() gives zeros.
 #ifndef B200JK_EMULATE
-// per-stage device timers of the last b200jk_df_jk call: mark(tag) ... mark(-1) brackets one stage with CUDA events on the
-// stream, without host synchronisation; read() adds the brackets up once the stream is synchronised
 struct StageTimer {
     std::vector<cudaEvent_t> ev; std::vector<int> tag; size_t used = 0;
     ~StageTimer() { for (cudaEvent_t e : ev) cudaEventDestroy(e); }
     void start() { used = 0; tag.clear(); }
-    void mark(int t, cudaStream_t st)
+    void mark(int t, stream_t st)
     {
         if (used == ev.size()) { cudaEvent_t e; CK(cudaEventCreate(&e)); ev.push_back(e); }
         CK(cudaEventRecord(ev[used++], st));
         tag.push_back(t);
     }
-    void read(double* ms, int* n) const
+    void read(double* ms, int* n, int nstage) const
     {
-        for (int i = 0; i < B200JK_DF_NSTAGE; i++) { ms[i] = 0; n[i] = 0; }
+        for (int i = 0; i < nstage; i++) { ms[i] = 0; if (n) n[i] = 0; }
         for (size_t i = 0; i + 1 < used; i++) {
             if (tag[i] < 0) continue;
             float t = 0;
             CK(cudaEventElapsedTime(&t, ev[i], ev[i + 1]));
-            ms[tag[i]] += t; n[tag[i]]++;
+            ms[tag[i]] += t;
+            if (n) n[tag[i]]++;
         }
     }
+};
+#else
+struct StageTimer {
+    void start() {}
+    void mark(int, stream_t) {}
+    void read(double* ms, int* n, int nstage) const { for (int i = 0; i < nstage; i++) { ms[i] = 0; if (n) n[i] = 0; } }
 };
 #endif
 
@@ -1721,7 +1732,7 @@ static int df_jk_impl(b200jk_handle h, const double* dm, int n_dm, int nao, cons
         float ms = 0;
         CK(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
         h->stats.ms_kernels = ms;
-        d->timer.read(d->stage_ms, d->stage_n);
+        d->timer.read(d->stage_ms, d->stage_n, B200JK_DF_NSTAGE);
         d->rows.read_times();
 #endif
         h->stats.ms_total = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();

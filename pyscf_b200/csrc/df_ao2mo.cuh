@@ -10,12 +10,15 @@
 // stay resident.
 // Stage 2: out[ij, kl] = sum_P L[P, ij] L'[P, kl] in bands of output rows; each band is copied to the caller through pinned
 // staging on the copy stream while the next band is computed.  With identical pairs the tiles above the diagonal of a band's
-// diagonal block are skipped and mirrored on the device (one band: half of the output).  get_eri is stage 2 with L = L' = B.
+// diagonal block are skipped and mirrored on the device (one band: half of the output).  get_eri is stage 2 with L = L' = B,
+// every band over all local rows by the same walk (host rows block by block, each block added).
 //
 // All three products run on ONE FP64 GEMM core on the tensor cores: DMMA.8x8x4 through nvcuda::wmma, CTA tile 64 x 64 x 16,
 // four warps of 32 x 32, operands fetched into registers one k step ahead by element loaders (packed-symmetric rows, plain and
-// transposed strided matrices).  The emulation build runs the same CTA code, thread by thread and warp by warp, on a host model
-// of the fragment operations.
+// transposed strided matrices) in one k loop, which DF-MP2's pair kernel and DF-RPA's Pi kernel run as well.  The emulation
+// build runs the same CTA code, thread by thread and warp by warp, on a host model of the fragment operations.
+// This file also holds what the four entry points on the tensor share: the call harness (MoCall), stage 1 (half_transform),
+// the active-spin parser of DF-MP2 and DF-RPA and the one-CTA tree sum.
 #include <thread>
 #ifndef B200JK_EMULATE
 #include <mma.h>
@@ -136,31 +139,80 @@ AO_D void epilogue(const G& g, const double* sm, long m0, long n0, int t)
     }
 }
 
+AO_D void red_step(double* red, int t, int s, int T) { if (t < s) { red[t] += red[t + s]; red[T + t] += red[T + t + s]; } }
+
+// A-operand hook of the k loop: at(k0, t) when thread t fetches k step k0, apply(ra) to its A operand of that step at the put
+struct NoHook {
+    AO_D void at(long, int) {}
+    AO_D void apply(double*) const {}
+};
+
+constexpr int RT = 256;     // threads of tree_sum
+
 #ifndef B200JK_EMULATE
+// One group of four warps (thread t of NT): c = sum over the k steps k0 = k_first, k_first + k_step, ... < k_end of the tile
+// (m0, n0) of g (steps past g.K read zeros), the operands staged through sm.  Every thread of the CTA must run the same number
+// of steps: each step has two barriers.
+template <class G, class H>
+AO_D void k_loop(const G& g, long m0, long n0, long k_first, long k_step, long k_end, double* sm, int t, H& hook,
+                 fr::C (&c)[4][4])
+{
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) fr::zero(c[i][j]);
+    double ra[PER_T], rb[PER_T];
+    fetch(g, m0, n0, k_first, t, ra, rb);
+    hook.at(k_first, t);
+    for (long k0 = k_first; k0 < k_end; k0 += k_step) {
+        hook.apply(ra);
+        put<G>(sm, t, ra, rb);
+        __syncthreads();
+        if (k0 + k_step < k_end) {     // next k step in flight during the MMAs
+            fetch(g, m0, n0, k0 + k_step, t, ra, rb);
+            hook.at(k0 + k_step, t);
+        }
+        warp_mma(sm, t >> 5, c);
+        __syncthreads();
+    }
+}
+
 template <class G>
 __global__ void __launch_bounds__(NT) f64gemm_kernel(G g, long n_base)
 {
     __shared__ __align__(128) double sm[SMEM];
     const long m0 = (long)blockIdx.x * BM, n0 = n_base + (long)blockIdx.y * BN;
     if (skipped(g, m0, n0)) return;
-    const int t = threadIdx.x, w = t >> 5;
+    const int t = threadIdx.x;
     fr::C c[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; i++)
-#pragma unroll
-        for (int j = 0; j < 4; j++) fr::zero(c[i][j]);
-    double ra[PER_T], rb[PER_T];
-    fetch(g, m0, n0, 0, t, ra, rb);
-    for (long k0 = 0; k0 < g.K; k0 += BK) {
-        put<G>(sm, t, ra, rb);
-        __syncthreads();
-        if (k0 + BK < g.K) fetch(g, m0, n0, k0 + BK, t, ra, rb);     // next k step in flight during the MMAs
-        warp_mma(sm, w, c);
-        __syncthreads();
-    }
-    warp_store(sm, w, c);
+    NoHook hk;
+    k_loop(g, m0, n0, 0, BK, g.K, sm, t, hk, c);
+    warp_store(sm, t >> 5, c);
     __syncthreads();
     epilogue(g, sm, m0, n0, t);
+}
+
+// one CTA of RT threads: out[0, 1] = the two sums over the shares share(t, a, b) of its threads, added in a fixed tree
+template <class F>
+__global__ void __launch_bounds__(RT) tree_sum_kernel(F share, double* out)
+{
+    __shared__ double red[2 * RT];
+    const int t = threadIdx.x;
+    double a = 0.0, b = 0.0;
+    share(t, a, b);
+    red[t] = a; red[RT + t] = b;
+    __syncthreads();
+    for (int s = RT / 2; s > 0; s >>= 1) {
+        red_step(red, t, s, RT);
+        __syncthreads();
+    }
+    if (t == 0) { out[0] = red[0]; out[1] = red[RT]; }
+}
+template <class F>
+static void tree_sum(const F& share, double* out, cudaStream_t s)
+{
+    tree_sum_kernel<F><<<1, RT, 0, s>>>(share, out);
+    CK(cudaGetLastError());
 }
 template <class G>
 static void gemm(const G& g, cudaStream_t s)
@@ -173,26 +225,60 @@ static void gemm(const G& g, cudaStream_t s)
     CK(cudaGetLastError());
 }
 #else
+// the device k_loop, thread by thread and warp by warp on the host model of the fragments: c[w] of warp w, hook copied per thread
+typedef fr::C Acc[4][4];
+template <class G, class H>
+static void k_loop(const G& g, long m0, long n0, long k_first, long k_step, long k_end, double* sm, const H& hook, Acc* c)
+{
+    std::vector<double> ra(NT * PER_T), rb(NT * PER_T);
+    std::vector<H> hk(NT, hook);
+    for (int w = 0; w < 4; w++)
+        for (int i = 0; i < 4; i++)
+            for (int j = 0; j < 4; j++) fr::zero(c[w][i][j]);
+    for (int t = 0; t < NT; t++) {
+        fetch(g, m0, n0, k_first, t, &ra[t * PER_T], &rb[t * PER_T]);
+        hk[t].at(k_first, t);
+    }
+    for (long k0 = k_first; k0 < k_end; k0 += k_step) {
+        for (int t = 0; t < NT; t++) {
+            hk[t].apply(&ra[t * PER_T]);
+            put<G>(sm, t, &ra[t * PER_T], &rb[t * PER_T]);
+        }
+        if (k0 + k_step < k_end)
+            for (int t = 0; t < NT; t++) {
+                fetch(g, m0, n0, k0 + k_step, t, &ra[t * PER_T], &rb[t * PER_T]);
+                hk[t].at(k0 + k_step, t);
+            }
+        for (int w = 0; w < 4; w++) warp_mma(sm, w, c[w]);
+    }
+}
+
 template <class G>
 static void gemm(const G& g, stream_t)
 {
-    std::vector<double> sm(SMEM), ra(NT * PER_T), rb(NT * PER_T);
-    std::vector<fr::C> cw(4 * 16);
+    std::vector<double> sm(SMEM);
+    Acc c[4];
     for (long m0 = 0; m0 < g.M; m0 += BM)
         for (long n0 = 0; n0 < g.N; n0 += BN) {
             if (skipped(g, m0, n0)) continue;
-            fr::C(*c)[4][4] = reinterpret_cast<fr::C(*)[4][4]>(cw.data());
-            for (fr::C& x : cw) fr::zero(x);
-            for (int t = 0; t < NT; t++) fetch(g, m0, n0, 0, t, &ra[t * PER_T], &rb[t * PER_T]);
-            for (long k0 = 0; k0 < g.K; k0 += BK) {
-                for (int t = 0; t < NT; t++) put<G>(sm.data(), t, &ra[t * PER_T], &rb[t * PER_T]);
-                if (k0 + BK < g.K)
-                    for (int t = 0; t < NT; t++) fetch(g, m0, n0, k0 + BK, t, &ra[t * PER_T], &rb[t * PER_T]);
-                for (int w = 0; w < 4; w++) warp_mma(sm.data(), w, c[w]);
-            }
+            k_loop(g, m0, n0, 0, BK, g.K, sm.data(), NoHook{}, c);
             for (int w = 0; w < 4; w++) warp_store(sm.data(), w, c[w]);
             for (int t = 0; t < NT; t++) epilogue(g, sm.data(), m0, n0, t);
         }
+}
+
+template <class F>
+static void tree_sum(const F& share, double* out, stream_t)
+{
+    std::vector<double> red(2 * RT);
+    for (int t = 0; t < RT; t++) {
+        double a = 0.0, b = 0.0;
+        share(t, a, b);
+        red[t] = a; red[RT + t] = b;
+    }
+    for (int s = RT / 2; s > 0; s >>= 1)
+        for (int t = 0; t < RT; t++) red_step(red.data(), t, s, RT);
+    out[0] = red[0]; out[1] = red[RT];
 }
 #endif
 
@@ -379,9 +465,87 @@ static void ao2mo_check_fit(double need, const char* what)
 #endif
 }
 
+// One call of an entry point that reads the resident tensor (ao2mo, get_ao_eri, DF-MP2, DF-RPA).  The constructor checks that
+// the tensor is built and not sharded (why: the caller's reason), selects the device and stream and starts the host clock.
+// finish() synchronises with a check, so that an asynchronous fault is reported, frees the buffers and returns the host ms;
+// the destructor frees what is still owned after an unchecked synchronisation, so that an error path cannot throw again.
+struct MoCall {
+    DFState* d;
+    stream_t st = 0;
+    std::vector<void*> owned;
+    std::chrono::steady_clock::time_point t0;
+
+    MoCall(b200jk_handle h, const char* fn, const char* why = "") : d(h->df)
+    {
+        if (!d || !d->d_cderi) throw std::runtime_error(std::string("call b200jk_df_build (or b200jk_df_set_cderi) before ") + fn);
+        if (d->build_world != 1) throw std::runtime_error(std::string(fn) + ": a sharded tensor is not supported" + why);
+#ifndef B200JK_EMULATE
+        CK(cudaSetDevice(h->device));
+        st = h->stream;
+#endif
+        t0 = std::chrono::steady_clock::now();
+    }
+    ~MoCall()
+    {
+#ifndef B200JK_EMULATE
+        cudaDeviceSynchronize();
+#endif
+        for (void* p : owned) dev_free(p);
+    }
+    void* alloc(size_t bytes)
+    {
+        void* p = dev_alloc(bytes);
+        owned.push_back(p);
+        return p;
+    }
+    void free(void* p)
+    {
+        dev_sync();
+        owned.erase(std::find(owned.begin(), owned.end(), p));
+        dev_free(p);
+    }
+    double finish()
+    {
+        dev_sync();
+        for (void* p : owned) dev_free(p);
+        owned.clear();
+        return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    }
+};
+
+// n stage times of the last call, from the DFState array src of N, into ms (zeros past N)
+template <int N>
+static int mo_times(b200jk_handle h, double (DFState::*src)[N], double* ms, int n)
+{
+    if (!h || !h->df || !ms) { set_err(h, "call b200jk_df_build first"); return 1; }
+    for (int i = 0; i < n; i++) ms[i] = i < N ? (h->df->*src)[i] : 0.0;
+    return 0;
+}
+
 // One coefficient pair of stage 1: host sets c[0] [nao][n[0]] and c[1] [nao][n[1]], their device copies dc, and the output
 // L[P][nij] (s2: i >= j at i(i+1)/2 + j, else i n[1] + j) over the local rows P.
 struct HalfPair { const double* c[2]; int n[2]; int s2; long nij; double* L; double* dc[2]; };
+
+// The spins of an occupied / virtual calculation (DF-MP2, DF-RPA) with orbitals on both sides: their stage-1 pairs (C_occ,
+// C_vir) in spin order, pr_of[s] = index in pr (-1: inactive) and the largest set contracted first.  e0, e1: the per-spin
+// arrays the caller needs of an active spin.
+struct ActiveSpins {
+    HalfPair pr[2];
+    int npr = 0, pr_of[2] = {-1, -1}, na_max = 1;
+    ActiveSpins(int nspin, const double* const* c_occ, const int* nocc, const double* const* c_vir, const int* nvir,
+                const double* const* e0, const double* const* e1)
+    {
+        for (int s = 0; s < nspin; s++) {
+            if (nocc[s] < 0 || nvir[s] < 0) throw std::runtime_error("bad arguments: negative orbital count");
+            if (nocc[s] == 0 || nvir[s] == 0) continue;
+            if (!c_occ[s] || !c_vir[s] || !e0[s] || !e1[s]) throw std::runtime_error("bad arguments");
+            pr[npr] = HalfPair{{c_occ[s], c_vir[s]}, {nocc[s], nvir[s]}, 0, (long)nocc[s] * nvir[s], nullptr, {nullptr, nullptr}};
+            na_max = std::max(na_max, std::min(nocc[s], nvir[s]));
+            pr_of[s] = npr++;
+        }
+    }
+    bool active(int s) const { return pr_of[s] >= 0; }
+};
 
 // tensor rows per stage-1 block: Y of a block at most 512 MiB; na_max = largest set contracted first
 static int half_block_rows(int nrow, int nao, int na_max)
@@ -389,23 +553,28 @@ static int half_block_rows(int nrow, int nao, int na_max)
     return (int)std::max<long>(1, std::min<long>(std::max(nrow, 1), (512L << 20) / ((long)nao * na_max * 8)));
 }
 
-// Stage 1 on the compute stream: L of every pair in pr[0, npr) from all local rows (device rows in place, host rows through the
-// staging buffers), in blocks of rb rows through d_Y [rb][nao][na_max].  Returns the device ms of the GEMMs.
-static double half_transform(DFState* d, int nao, stream_t st, HalfPair* pr, int npr, double* d_Y, int rb)
+// Stage 1 on the compute stream: allocates L and the device coefficients of every pair in pr[0, npr) through the call,
+// uploads the coefficients and fills L from all local rows (device rows in place, host rows through the staging buffers), in
+// blocks of rb rows through a temporary Y [rb][nao][na_max] that is freed again.  Returns the device ms of the GEMMs.
+static double half_transform(MoCall& c, int nao, HalfPair* pr, int npr, int rb, int na_max)
 {
-    const int nrow = d->nrow;
+    if (npr == 0) return 0.0;
+    DFState* d = c.d;
+    const stream_t st = c.st;
     const long ld = d->ncol;
     const int* col_of = d->d_col_of;
-    double ms1 = 0.0;
-#ifndef B200JK_EMULATE
-    std::vector<cudaEvent_t> tev;
-    auto mark = [&]() { cudaEvent_t e; CK(cudaEventCreate(&e)); CK(cudaEventRecord(e, st)); tev.push_back(e); };
-#else
-    auto mark = [&]() {};
-#endif
+    for (int q = 0; q < npr; q++) {
+        pr[q].L = (double*)c.alloc((size_t)std::max(d->nrow, 1) * pr[q].nij * 8);
+        for (int s = 0; s < 2; s++) {
+            pr[q].dc[s] = (double*)c.alloc((size_t)nao * pr[q].n[s] * 8);
+            h2d(pr[q].dc[s], pr[q].c[s], (size_t)nao * pr[q].n[s] * 8, st);
+        }
+    }
+    double* d_Y = (double*)c.alloc((size_t)rb * nao * na_max * 8);
+    StageTimer tm;
     // ---- stage 1 on the rows [r0, r0 + nr) at src
     auto half = [&](const double* src, int r0, int nr) {
-        mark();
+        tm.mark(0, st);
         for (int q = 0; q < npr; q++) {
             HalfPair& p = pr[q];
             const int f = p.n[0] <= p.n[1] ? 0 : 1;     // the smaller set is contracted first
@@ -417,26 +586,15 @@ static double half_transform(DFState* d, int nao, stream_t st, HalfPair* pr, int
                                                                      {p.L + (size_t)r0 * p.nij, p.nij, na, p.n[1], f == 1, p.s2}, 0, 0, 0};
             ao2mo::gemm(g2, st);
         }
-        mark();
+        tm.mark(-1, st);
     };
-    try {
-        d->rows.walk(d->d_cderi, 0, nrow, std::min(rb, d->rows.stage_rows), false, st, [&](const double* src, int r0, int nr) {
-            for (int q = 0; q < nr; q += rb) half(src + (size_t)q * ld, r0 + q, std::min(rb, nr - q));
-        });
-#ifndef B200JK_EMULATE
-        CK(cudaStreamSynchronize(st));
-        for (size_t i = 0; i + 1 < tev.size(); i += 2) { float t = 0; CK(cudaEventElapsedTime(&t, tev[i], tev[i + 1])); ms1 += t; }
-#endif
-    } catch (...) {
-#ifndef B200JK_EMULATE
-        for (cudaEvent_t e : tev) cudaEventDestroy(e);
-#endif
-        throw;
-    }
-#ifndef B200JK_EMULATE
-    for (cudaEvent_t e : tev) cudaEventDestroy(e);
-#endif
-    return ms1;
+    d->rows.walk(d->d_cderi, 0, d->nrow, std::min(rb, d->rows.stage_rows), false, st, [&](const double* src, int r0, int nr) {
+        for (int q = 0; q < nr; q += rb) half(src + (size_t)q * ld, r0 + q, std::min(rb, nr - q));
+    });
+    c.free(d_Y);
+    double ms = 0.0;
+    tm.read(&ms, nullptr, 1);
+    return ms;
 }
 
 extern "C" int b200jk_df_ao2mo(b200jk_handle h, const double* c1, int n1, const double* c2, int n2, int s2_12, const double* c3,
@@ -444,21 +602,13 @@ extern "C" int b200jk_df_ao2mo(b200jk_handle h, const double* c1, int n1, const 
 {
     if (!h) return 1;
     try {
-        DFState* d = h->df;
-        if (!d || !d->d_cderi) throw std::runtime_error("call b200jk_df_build (or b200jk_df_set_cderi) before b200jk_df_ao2mo");
-        if (d->build_world != 1) throw std::runtime_error("b200jk_df_ao2mo: a sharded tensor is not supported");
+        MoCall c(h, "b200jk_df_ao2mo");
+        DFState* d = c.d;
         const bool same = c3 == nullptr;
         if (same) { c3 = c1; n3 = n1; c4 = c2; n4 = n2; s2_34 = s2_12; }
         if (!c1 || !c2 || !c4 || !out || n1 < 1 || n2 < 1 || n3 < 1 || n4 < 1) throw std::runtime_error("bad arguments");
         if ((s2_12 && n1 != n2) || (s2_34 && n3 != n4)) throw std::runtime_error("an s2 pair needs two sets of equal size");
-        auto t_start = std::chrono::steady_clock::now();
         const int nao = h->nsph, nrow = d->nrow;
-#ifndef B200JK_EMULATE
-        CK(cudaSetDevice(h->device));
-        cudaStream_t st = h->stream;
-#else
-        stream_t st = 0;
-#endif
         HalfPair pr[2] = {{{c1, c2}, {n1, n2}, s2_12, 0, nullptr, {nullptr, nullptr}},
                           {{c3, c4}, {n3, n4}, s2_34, 0, nullptr, {nullptr, nullptr}}};
         const int npr = same ? 1 : 2;
@@ -472,40 +622,22 @@ extern "C" int b200jk_df_ao2mo(b200jk_handle h, const double* c1, int n1, const 
         const long band = ao2mo_band_rows(d, nij, nkl * 8);
         ao2mo_check_fit(8.0 * ((double)nrow * (nij + (same ? 0 : nkl)) + (double)rb * nao * na_max + 2.0 * band * nkl),
                         "the half-transformed integrals L[naux, nij] (and L[naux, nkl]) with their work buffers");
-        std::vector<double*> owned;
-        auto alloc = [&](size_t n) { double* p = (double*)dev_alloc(n * 8); owned.push_back(p); return p; };
-        try {
-            for (int q = 0; q < npr; q++) {
-                pr[q].L = alloc((size_t)std::max(nrow, 1) * pr[q].nij);
-                for (int s = 0; s < 2; s++) {
-                    pr[q].dc[s] = alloc((size_t)nao * pr[q].n[s]);
-                    h2d(pr[q].dc[s], pr[q].c[s], (size_t)nao * pr[q].n[s] * 8, st);
-                }
-            }
-            double* d_Y = alloc((size_t)rb * nao * na_max);
-            const double ms1 = half_transform(d, nao, st, pr, npr, d_Y, rb);
-            double ms2 = 0.0;
-            // ---- stage 2: bands of output rows [r0, r1)
-            const double* Lij = pr[0].L;
-            const double* Lkl = pr[npr - 1].L;
-            const int nbands = (int)((nij + band - 1) / band);
-            ao2mo::band_pipeline(d, st, nbands, (size_t)band * nkl * 8, [&](int b, double* buf) -> size_t {
-                const long r0 = (long)b * band, r1 = std::min(nij, r0 + band);
-                ao2mo::Gemm<ao2mo::TransA, ao2mo::RowsB, ao2mo::RowsSt> g{r1 - r0, nkl, nrow, {Lij + r0, nij}, {Lkl, nkl}, {buf, nkl},
-                                                                          same ? 1 : 0, r0, r1};
-                ao2mo::gemm(g, st);
-                if (same) { ao2mo::MirrorBandFn mf{buf, nkl, r0, r1 - r0}; launch_1d((r1 - r0) * (r1 - r0), mf, st); }
-                return (size_t)(r1 - r0) * nkl * 8;
-            }, [&](int b, const void* src, size_t n) { ao2mo::par_memcpy(out + (size_t)b * band * nkl, src, n); }, ms2);
-            d->ao2mo_ms[0] = ms1; d->ao2mo_ms[1] = ms2;
-        } catch (...) {
-            dev_sync();
-            for (double* p : owned) dev_free(p);
-            throw;
-        }
-        dev_sync();
-        for (double* p : owned) dev_free(p);
-        d->ao2mo_ms[2] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+        const double ms1 = half_transform(c, nao, pr, npr, rb, na_max);
+        double ms2 = 0.0;
+        // ---- stage 2: bands of output rows [r0, r1)
+        const double* Lij = pr[0].L;
+        const double* Lkl = pr[npr - 1].L;
+        const int nbands = (int)((nij + band - 1) / band);
+        ao2mo::band_pipeline(d, c.st, nbands, (size_t)band * nkl * 8, [&](int b, double* buf) -> size_t {
+            const long r0 = (long)b * band, r1 = std::min(nij, r0 + band);
+            ao2mo::Gemm<ao2mo::TransA, ao2mo::RowsB, ao2mo::RowsSt> g{r1 - r0, nkl, nrow, {Lij + r0, nij}, {Lkl, nkl}, {buf, nkl},
+                                                                      same ? 1 : 0, r0, r1};
+            ao2mo::gemm(g, c.st);
+            if (same) { ao2mo::MirrorBandFn mf{buf, nkl, r0, r1 - r0}; launch_1d((r1 - r0) * (r1 - r0), mf, c.st); }
+            return (size_t)(r1 - r0) * nkl * 8;
+        }, [&](int b, const void* src, size_t n) { ao2mo::par_memcpy(out + (size_t)b * band * nkl, src, n); }, ms2);
+        d->ao2mo_ms[0] = ms1; d->ao2mo_ms[1] = ms2;
+        d->ao2mo_ms[2] = c.finish();
     } catch (std::exception& e) { set_err(h, e.what()); return 2; }
     return 0;
 }
@@ -514,20 +646,11 @@ extern "C" int b200jk_df_get_ao_eri(b200jk_handle h, double* out)
 {
     if (!h) return 1;
     try {
-        DFState* d = h->df;
-        if (!d || !d->d_cderi) throw std::runtime_error("call b200jk_df_build (or b200jk_df_set_cderi) before b200jk_df_get_ao_eri");
-        if (d->build_world != 1) throw std::runtime_error("b200jk_df_get_ao_eri: a sharded tensor is not supported");
+        MoCall c(h, "b200jk_df_get_ao_eri");
+        DFState* d = c.d;
         if (!out) throw std::runtime_error("bad arguments");
-        auto t_start = std::chrono::steady_clock::now();
         const long npair = d->npair, ld = d->ncol;
         const int* col_of = d->d_col_of;
-        const int nrow = d->nrow, n_dev = d->rows.n_dev;
-#ifndef B200JK_EMULATE
-        CK(cudaSetDevice(h->device));
-        cudaStream_t st = h->stream;
-#else
-        stream_t st = 0;
-#endif
         // bands of s8 rows [r0, r1), each at most the bytes of ao2mo_band_rows(npair rows of npair columns)
         const long band = ao2mo_band_rows(d, npair, npair * 8);
         std::vector<long> rows{0};
@@ -539,25 +662,18 @@ extern "C" int b200jk_df_get_ao_eri(b200jk_handle h, double* out)
         }
         ao2mo_check_fit(16.0 * band * npair, "the output bands of get_ao_eri");
         double ms2 = 0.0;
-        ao2mo::band_pipeline(d, st, (int)rows.size() - 1, (size_t)band * npair * 8, [&](int b, double* buf) -> size_t {
+        ao2mo::band_pipeline(d, c.st, (int)rows.size() - 1, (size_t)band * npair * 8, [&](int b, double* buf) -> size_t {
             const long r0 = rows[b], r1 = rows[b + 1];
-            auto part = [&](const double* src, int nr, int acc) {
+            // every local row block adds to the band; the first one (device rows, or the first host block) stores
+            d->rows.walk(d->d_cderi, 0, d->nrow, d->rows.stage_rows, false, c.st, [&](const double* src, int a0, int nr) {
                 ao2mo::Gemm<ao2mo::PackedColsA, ao2mo::PackedColsB, ao2mo::TriBandSt> g{r1 - r0, r1, nr, {src, ld, col_of, r0},
-                                                                                        {src, ld, col_of}, {buf, r0, acc}, 1, r0, r1};
-                ao2mo::gemm(g, st);
-            };
-            part(d->d_cderi, n_dev, 0);
-            // host rows (a tensor larger than the device): staged block by block and added
-            for (int a = n_dev; a < nrow; a += d->rows.stage_rows) {
-                const int nr = std::min(d->rows.stage_rows, nrow - a);
-                h2d(d->rows.d_stage[0], d->rows.host_row(a), (size_t)nr * ld * 8, st);
-                part(d->rows.d_stage[0], nr, 1);
-            }
+                                                                                        {src, ld, col_of}, {buf, r0, a0 > 0}, 1, r0, r1};
+                ao2mo::gemm(g, c.st);
+            });
             return (size_t)(r1 * (r1 + 1) / 2 - r0 * (r0 + 1) / 2) * 8;
         }, [&](int b, const void* src, size_t n) { ao2mo::par_memcpy(out + rows[b] * (rows[b] + 1) / 2, src, n); }, ms2);
-        dev_sync();
         d->ao2mo_ms[0] = 0.0; d->ao2mo_ms[1] = ms2;
-        d->ao2mo_ms[2] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+        d->ao2mo_ms[2] = c.finish();
     } catch (std::exception& e) { set_err(h, e.what()); return 2; }
     return 0;
 }
@@ -570,9 +686,4 @@ extern "C" int b200jk_df_set_ao2mo_tile(b200jk_handle h, int max_rows)
     return 0;
 }
 
-extern "C" int b200jk_df_ao2mo_times(b200jk_handle h, double* ms, int n)
-{
-    if (!h || !h->df || !ms) { set_err(h, "call b200jk_df_build first"); return 1; }
-    for (int i = 0; i < n; i++) ms[i] = i < 3 ? h->df->ao2mo_ms[i] : 0.0;
-    return 0;
-}
+extern "C" int b200jk_df_ao2mo_times(b200jk_handle h, double* ms, int n) { return mo_times(h, &DFState::ao2mo_ms, ms, n); }

@@ -20,12 +20,11 @@
 // the band size, on where the tensor rows live or on the launch order: two calls give the same bits.
 
 namespace mp2k {
-using ao2mo::BM; using ao2mo::BN; using ao2mo::BK; using ao2mo::NT; using ao2mo::LDC; using ao2mo::PER_T;
+using ao2mo::BM; using ao2mo::BN; using ao2mo::BK; using ao2mo::NT; using ao2mo::LDC; using ao2mo::RT;
 using ao2mo::SM_AB; using ao2mo::SM_C;
 
 constexpr int SMEM = 2 * SM_C;      // two staged C tiles; the operand tiles of both products (2 SM_AB) sit below them
 static_assert(2 * SM_AB <= SMEM, "operands of both products fit in the C staging");
-constexpr int RT = 256;             // threads of the final sum
 
 struct NoSt {};
 typedef ao2mo::Gemm<ao2mo::TransA, ao2mo::RowsB, NoSt> PairGemm;   // a(m, k) = L_i[k, m], b(k, n) = L_j[k, n]
@@ -68,8 +67,6 @@ AO_D void epi_tile(const Job& jb, const double* X, const double* Y, long R0, lon
     }
 }
 
-AO_D void red_step(double* red, int t, int s, int T) { if (t < s) { red[t] += red[t + s]; red[T + t] += red[T + t + s]; } }
-
 // CTA (pair p, tile pair tp) of T threads after its products: the epilogue of thread t; the tiles are staged at sm (V[A, B])
 // and, when two, at sm + SM_C (V[B, A])
 AO_D void cta_epilogue(const Job& jb, const double* sm, long p, int i, int j, long A0, long B0, bool two, int t, int T, double* red)
@@ -90,23 +87,21 @@ AO_D void cta_store(const Job& jb, const double* red, long p, int tp, int i, int
 // threads of a CTA: one group of four warps per accumulator
 AO_D constexpr int cta_threads(int os) { return os ? NT : 2 * NT; }
 // k steps of group grp: a diagonal same-spin tile pair (split) gives the two groups alternate steps (grp, grp + 2, ...) of its
-// one product, else each group takes them all
-AO_D void k_plan(bool split, int grp, long K, long& k_first, long& k_step, long& n_iter)
+// one product, else each group takes them all; both groups run the same number of steps (the last one of group 1 may be past K)
+AO_D void k_plan(bool split, int grp, long K, long& k_first, long& k_step, long& k_end)
 {
     const long nk = (K + BK - 1) / BK;
     k_first = split ? grp * BK : 0;
     k_step = split ? 2 * BK : BK;
-    n_iter = split ? (nk + 1) / 2 : nk;
+    k_end = k_first + (split ? (nk + 1) / 2 : nk) * k_step;
 }
 // thread t (of T) of the sum of the two staged halves of a split product into the first tile
 AO_D void add_halves(double* sm, int t, int T) { for (int e = t; e < BM * LDC; e += T) sm[e] += sm[SM_C + e]; }
-// thread t of the final pass: its strided share of n partial (ed, ex)
-AO_D void sum_share(const double* part, long n, int t, double* red)
-{
-    double a = 0.0, b = 0.0;
-    for (long q = t; q < n; q += RT) { a += part[2 * q]; b += part[2 * q + 1]; }
-    red[t] = a; red[RT + t] = b;
-}
+// thread t of the final sum: its strided share of n partial (ed, ex)
+struct PartShare {
+    const double* part; long n;
+    AO_D void operator()(int t, double& a, double& b) const { for (long q = t; q < n; q += RT) { a += part[2 * q]; b += part[2 * q + 1]; } }
+};
 
 #ifndef B200JK_EMULATE
 // group 0 (threads [0, NT)) accumulates V[A, B], group 1 V[B, A]; on a diagonal tile pair they split the k steps of V[A, A]
@@ -121,28 +116,14 @@ __global__ void __launch_bounds__(cta_threads(OS)) mp2_pair_kernel(Job jb, long 
     const int i = jb.pairs[2 * p], j = jb.pairs[2 * p + 1];
     const long A0 = (long)jb.tiles[2 * tp] * BM, B0 = (long)jb.tiles[2 * tp + 1] * BN;
     const bool two = !OS && A0 != B0, split = !OS && A0 == B0;
-    const int t = threadIdx.x, grp = t / NT, tg = t % NT, w = tg >> 5;
-    const long m0 = grp ? B0 : A0, n0 = grp ? A0 : B0;
-    double* smg = sm + grp * SM_AB;
+    const int t = threadIdx.x, grp = t / NT, tg = t % NT;
     const PairGemm g = pair_gemm(jb, i, j);
     ao2mo::fr::C c[4][4];
-#pragma unroll
-    for (int a = 0; a < 4; a++)
-#pragma unroll
-        for (int b = 0; b < 4; b++) ao2mo::fr::zero(c[a][b]);
-    double ra[PER_T], rb[PER_T];
-    long kf, ks, ni;
-    k_plan(split, grp, g.K, kf, ks, ni);
-    ao2mo::fetch(g, m0, n0, kf, tg, ra, rb);
-    for (long it = 0; it < ni; it++) {
-        const long k0 = kf + it * ks;
-        ao2mo::put<PairGemm>(smg, tg, ra, rb);
-        __syncthreads();
-        if (it + 1 < ni) ao2mo::fetch(g, m0, n0, k0 + ks, tg, ra, rb);     // next k step in flight during the MMAs
-        ao2mo::warp_mma(smg, w, c);
-        __syncthreads();
-    }
-    ao2mo::warp_store(sm + grp * SM_C, w, c);
+    ao2mo::NoHook hk;
+    long kf, ks, ke;
+    k_plan(split, grp, g.K, kf, ks, ke);
+    ao2mo::k_loop(g, grp ? B0 : A0, grp ? A0 : B0, kf, ks, ke, sm + grp * SM_AB, tg, hk, c);
+    ao2mo::warp_store(sm + grp * SM_C, tg >> 5, c);
     __syncthreads();
     if (split) {
         add_halves(sm, t, T);
@@ -151,23 +132,10 @@ __global__ void __launch_bounds__(cta_threads(OS)) mp2_pair_kernel(Job jb, long 
     cta_epilogue(jb, sm, p, i, j, A0, B0, two, t, T, red);
     __syncthreads();
     for (int s = T / 2; s > 0; s >>= 1) {
-        red_step(red, t, s, T);
+        ao2mo::red_step(red, t, s, T);
         __syncthreads();
     }
     if (t == 0) cta_store(jb, red, p, tp, i, j, T);
-}
-
-__global__ void __launch_bounds__(RT) mp2_sum_kernel(const double* part, long n, double* out)
-{
-    __shared__ double red[2 * RT];
-    const int t = threadIdx.x;
-    sum_share(part, n, t, red);
-    __syncthreads();
-    for (int s = RT / 2; s > 0; s >>= 1) {
-        red_step(red, t, s, RT);
-        __syncthreads();
-    }
-    if (t == 0) { out[0] = red[0]; out[1] = red[RT]; }
 }
 
 // pairs [p0, p1) of the job, every tile pair
@@ -184,61 +152,34 @@ static void pair_launch(const Job& jb, long p0, long p1, cudaStream_t s)
     }
     CK(cudaGetLastError());
 }
-static void sum_launch(const double* part, long n, double* out, cudaStream_t s)
-{
-    mp2_sum_kernel<<<1, RT, 0, s>>>(part, n, out);
-    CK(cudaGetLastError());
-}
 #else
-// the same CTA code, thread by thread and warp by warp, on the host model of the fragments
+// the same CTA code on the host model; the two groups of warps run one after the other (their operand tiles and accumulators
+// are disjoint until the stores)
 static void pair_launch(const Job& jb, long p0, long p1, stream_t)
 {
     const int T = cta_threads(jb.os);
-    std::vector<double> sm(SMEM), red(2 * T), ra(T * PER_T), rb(T * PER_T);
-    std::vector<ao2mo::fr::C> cw(2 * 4 * 16);
-    typedef ao2mo::fr::C Acc[4][4];
-    Acc* c = reinterpret_cast<Acc*>(cw.data());     // c[grp * 4 + w]
+    std::vector<double> sm(SMEM), red(2 * T);
+    ao2mo::Acc c[8];     // c[grp * 4 + w]
     for (long p = p0; p < p1; p++)
         for (int tp = 0; tp < jb.ntp; tp++) {
             const int i = jb.pairs[2 * p], j = jb.pairs[2 * p + 1];
             const long A0 = (long)jb.tiles[2 * tp] * BM, B0 = (long)jb.tiles[2 * tp + 1] * BN;
             const bool two = !jb.os && A0 != B0, split = !jb.os && A0 == B0;
-            const int ngrp = T / NT;
             const PairGemm g = pair_gemm(jb, i, j);
-            for (ao2mo::fr::C& x : cw) ao2mo::fr::zero(x);
-            long kf[2], ks = 0, ni = 0;
-            for (int grp = 0; grp < ngrp; grp++) {
-                k_plan(split, grp, g.K, kf[grp], ks, ni);
-                for (int tg = 0; tg < NT; tg++)
-                    ao2mo::fetch(g, grp ? B0 : A0, grp ? A0 : B0, kf[grp], tg, &ra[(grp * NT + tg) * PER_T], &rb[(grp * NT + tg) * PER_T]);
+            for (int grp = 0; grp < T / NT; grp++) {
+                long kf, ks, ke;
+                k_plan(split, grp, g.K, kf, ks, ke);
+                ao2mo::k_loop(g, grp ? B0 : A0, grp ? A0 : B0, kf, ks, ke, sm.data() + grp * SM_AB, ao2mo::NoHook{}, c + 4 * grp);
             }
-            for (long it = 0; it < ni; it++)
-                for (int grp = 0; grp < ngrp; grp++) {
-                    double* smg = sm.data() + grp * SM_AB;
-                    for (int tg = 0; tg < NT; tg++) ao2mo::put<PairGemm>(smg, tg, &ra[(grp * NT + tg) * PER_T], &rb[(grp * NT + tg) * PER_T]);
-                    if (it + 1 < ni)
-                        for (int tg = 0; tg < NT; tg++)
-                            ao2mo::fetch(g, grp ? B0 : A0, grp ? A0 : B0, kf[grp] + (it + 1) * ks, tg, &ra[(grp * NT + tg) * PER_T],
-                                         &rb[(grp * NT + tg) * PER_T]);
-                    for (int w = 0; w < 4; w++) ao2mo::warp_mma(smg, w, c[grp * 4 + w]);
-                }
-            for (int grp = 0; grp < ngrp; grp++)
+            for (int grp = 0; grp < T / NT; grp++)
                 for (int w = 0; w < 4; w++) ao2mo::warp_store(sm.data() + grp * SM_C, w, c[grp * 4 + w]);
             if (split)
                 for (int t = 0; t < T; t++) add_halves(sm.data(), t, T);
             for (int t = 0; t < T; t++) cta_epilogue(jb, sm.data(), p, i, j, A0, B0, two, t, T, red.data());
             for (int s = T / 2; s > 0; s >>= 1)
-                for (int t = 0; t < T; t++) red_step(red.data(), t, s, T);
+                for (int t = 0; t < T; t++) ao2mo::red_step(red.data(), t, s, T);
             cta_store(jb, red.data(), p, tp, i, j, T);
         }
-}
-static void sum_launch(const double* part, long n, double* out, stream_t)
-{
-    std::vector<double> red(2 * RT);
-    for (int t = 0; t < RT; t++) sum_share(part, n, t, red.data());
-    for (int s = RT / 2; s > 0; s >>= 1)
-        for (int t = 0; t < RT; t++) red_step(red.data(), t, s, RT);
-    out[0] = red[0]; out[1] = red[RT];
 }
 #endif
 
@@ -273,36 +214,13 @@ extern "C" int b200jk_df_mp2(b200jk_handle h, int nspin, const double* const* c_
 {
     if (!h) return 1;
     try {
-        DFState* d = h->df;
-        if (!d || !d->d_cderi) throw std::runtime_error("call b200jk_df_build (or b200jk_df_set_cderi) before b200jk_df_mp2");
-        if (d->build_world != 1)
-            throw std::runtime_error("b200jk_df_mp2: a sharded tensor is not supported (the pair energies are not linear in the "
-                                     "local rows)");
+        MoCall c(h, "b200jk_df_mp2", " (the pair energies are not linear in the local rows)");
+        DFState* d = c.d;
+        const stream_t st = c.st;
         if ((nspin != 1 && nspin != 2) || !c_occ || !nocc || !c_vir || !nvir || !e_occ || !e_vir || !e_out)
             throw std::runtime_error("bad arguments");
-        bool active[2] = {false, false};
-        for (int s = 0; s < nspin; s++) {
-            if (nocc[s] < 0 || nvir[s] < 0) throw std::runtime_error("bad arguments: negative orbital count");
-            active[s] = nocc[s] > 0 && nvir[s] > 0;
-            if (active[s] && (!c_occ[s] || !c_vir[s] || !e_occ[s] || !e_vir[s])) throw std::runtime_error("bad arguments");
-        }
-        auto t_start = std::chrono::steady_clock::now();
+        ActiveSpins sp(nspin, c_occ, nocc, c_vir, nvir, e_occ, e_vir);
         const int nao = h->nsph, nrow = d->nrow;
-#ifndef B200JK_EMULATE
-        CK(cudaSetDevice(h->device));
-        cudaStream_t st = h->stream;
-#else
-        stream_t st = 0;
-#endif
-        // stage-1 pairs (co, cv) of the active spins; pr_of[s] = index in pr
-        HalfPair pr[2];
-        int pr_of[2] = {-1, -1}, npr = 0, na_max = 1;
-        for (int s = 0; s < nspin; s++)
-            if (active[s]) {
-                pr[npr] = HalfPair{{c_occ[s], c_vir[s]}, {nocc[s], nvir[s]}, 0, (long)nocc[s] * nvir[s], nullptr, {nullptr, nullptr}};
-                na_max = std::max(na_max, std::min(nocc[s], nvir[s]));
-                pr_of[s] = npr++;
-            }
         // jobs: (spin of i, spin of j, opposite spin, t2 mode, caller's t2 block)
         struct JobSpec { int sa, sb, os, mode; double* t2; long npair, ntp; };
         std::vector<JobSpec> specs;
@@ -315,129 +233,91 @@ extern "C" int b200jk_df_mp2(b200jk_handle h, int nspin, const double* const* c_
         auto ntile = [](int nv) { return (long)(nv + ao2mo::BM - 1) / ao2mo::BM; };
         double need = 0.0, part_total = 0.0, band_max = 0.0;
         for (JobSpec& js : specs) {
-            if (!active[js.sa] || !active[js.sb]) continue;
+            if (!sp.active(js.sa) || !sp.active(js.sb)) continue;
             js.npair = js.os ? (long)nocc[js.sa] * nocc[js.sb] : (long)nocc[js.sa] * (nocc[js.sa] + 1) / 2;
             js.ntp = js.os ? ntile(nvir[js.sa]) * ntile(nvir[js.sb]) : ntile(nvir[js.sa]) * (ntile(nvir[js.sa]) + 1) / 2;
             part_total += 2.0 * js.npair * js.ntp;
             const long nvv = (long)nvir[js.sa] * nvir[js.sb];
             if (js.t2) band_max = std::max(band_max, (double)ao2mo_band_rows(d, js.npair, nvv * 8) * nvv);
         }
-        const int rb = half_block_rows(nrow, nao, na_max);
-        for (int q = 0; q < npr; q++) need += (double)nrow * pr[q].nij;
-        need += std::max((double)rb * nao * na_max, part_total + 2.0 * band_max);
+        const int rb = half_block_rows(nrow, nao, sp.na_max);
+        for (int q = 0; q < sp.npr; q++) need += (double)nrow * sp.pr[q].nij;
+        need += std::max((double)rb * nao * sp.na_max, part_total + 2.0 * band_max);
         ao2mo_check_fit(8.0 * need, "DF-MP2: the half-transformed integrals L[naux, nocc nvir] of each spin with their work buffers");
 
-        std::vector<void*> owned;
-        auto alloc = [&](size_t bytes) { void* p = dev_alloc(bytes); owned.push_back(p); return p; };
-        try {
-            double ms1 = 0.0, ms2 = 0.0;
-            if (npr > 0) {
-                for (int q = 0; q < npr; q++) {
-                    pr[q].L = (double*)alloc((size_t)std::max(nrow, 1) * pr[q].nij * 8);
-                    for (int s = 0; s < 2; s++) {
-                        pr[q].dc[s] = (double*)alloc((size_t)nao * pr[q].n[s] * 8);
-                        h2d(pr[q].dc[s], pr[q].c[s], (size_t)nao * pr[q].n[s] * 8, st);
-                    }
-                }
-                double* d_Y = (double*)dev_alloc((size_t)rb * nao * na_max * 8);
-                try { ms1 = half_transform(d, nao, st, pr, npr, d_Y, rb); } catch (...) { dev_sync(); dev_free(d_Y); throw; }
-                dev_sync();
-                dev_free(d_Y);
+        const double ms1 = half_transform(c, nao, sp.pr, sp.npr, rb, sp.na_max);
+        double ms2 = 0.0;
+        double* d_eo[2] = {nullptr, nullptr};
+        double* d_ev[2] = {nullptr, nullptr};
+        for (int s = 0; s < nspin; s++)
+            if (sp.active(s)) {
+                d_eo[s] = (double*)c.alloc((size_t)nocc[s] * 8);
+                d_ev[s] = (double*)c.alloc((size_t)nvir[s] * 8);
+                h2d(d_eo[s], e_occ[s], (size_t)nocc[s] * 8, st);
+                h2d(d_ev[s], e_vir[s], (size_t)nvir[s] * 8, st);
             }
-            double* d_eo[2] = {nullptr, nullptr};
-            double* d_ev[2] = {nullptr, nullptr};
-            for (int s = 0; s < nspin; s++)
-                if (active[s]) {
-                    d_eo[s] = (double*)alloc((size_t)nocc[s] * 8);
-                    d_ev[s] = (double*)alloc((size_t)nvir[s] * 8);
-                    h2d(d_eo[s], e_occ[s], (size_t)nocc[s] * 8, st);
-                    h2d(d_ev[s], e_vir[s], (size_t)nvir[s] * 8, st);
-                }
-            double* d_sums = (double*)alloc(2 * specs.size() * 8);
-            dev_zero(d_sums, 2 * specs.size() * 8, st);
-#ifndef B200JK_EMULATE
-            cudaEvent_t ev[2];
-            for (cudaEvent_t& e : ev) CK(cudaEventCreate(&e));
-#endif
-            std::vector<std::vector<int>> pair_lists(specs.size());
-            for (size_t k = 0; k < specs.size(); k++) {
-                const JobSpec& js = specs[k];
-                if (js.npair == 0) continue;
-                const int sa = js.sa, sb = js.sb, nva = nvir[sa], nvb = nvir[sb];
-                // pairs i-major (consecutive CTAs share L_i), tile pairs in row order
-                std::vector<int>& pl = pair_lists[k];
-                for (int i = 0; i < nocc[sa]; i++)
-                    for (int j = 0; j < (js.os ? nocc[sb] : i + 1); j++) { pl.push_back(i); pl.push_back(j); }
-                std::vector<int> tl;
-                for (int A = 0; A < ntile(nva); A++)
-                    for (int B = js.os ? 0 : A; B < ntile(nvb); B++) { tl.push_back(A); tl.push_back(B); }
-                int* d_pairs = (int*)alloc(pl.size() * 4);
-                int* d_tiles = (int*)alloc(tl.size() * 4);
-                h2d(d_pairs, pl.data(), pl.size() * 4, st);
-                h2d(d_tiles, tl.data(), tl.size() * 4, st);
-                double* d_part = (double*)alloc((size_t)js.npair * js.ntp * 2 * 8);
-                mp2k::Job jb{pr[pr_of[sa]].L, pr[pr_of[sb]].L, pr[pr_of[sa]].nij, pr[pr_of[sb]].nij, nva, nvb, nrow,
-                             d_eo[sa], d_eo[sb], d_ev[sa], d_ev[sb], d_pairs, d_tiles, (int)js.ntp, js.os, js.mode,
-                             nullptr, 0, d_part};
-                if (!js.t2) {
-#ifndef B200JK_EMULATE
-                    CK(cudaEventRecord(ev[0], st));
-#endif
-                    mp2k::pair_launch(jb, 0, js.npair, st);
-                    mp2k::sum_launch(d_part, js.npair * js.ntp, d_sums + 2 * k, st);
-#ifndef B200JK_EMULATE
-                    CK(cudaEventRecord(ev[1], st));
-                    CK(cudaEventSynchronize(ev[1]));
-                    float t = 0;
-                    CK(cudaEventElapsedTime(&t, ev[0], ev[1]));
-                    ms2 += t;
-#endif
-                } else {
-                    const long nvv = (long)nva * nvb, band = ao2mo_band_rows(d, js.npair, nvv * 8);
-                    const int nbands = (int)((js.npair + band - 1) / band);
-                    ao2mo::band_pipeline(d, st, nbands, (size_t)band * nvv * 8, [&](int b, double* buf) -> size_t {
-                        const long p0 = (long)b * band, p1 = std::min(js.npair, p0 + band);
-                        mp2k::Job jt = jb;
-                        jt.t2 = buf; jt.p0 = p0;
-                        mp2k::pair_launch(jt, p0, p1, st);
-                        if (b == nbands - 1) mp2k::sum_launch(d_part, js.npair * js.ntp, d_sums + 2 * k, st);
-                        return (size_t)(p1 - p0) * nvv * 8;
-                    }, [&](int b, const void* src, size_t n) {
-                        mp2k::scatter_t2(pl.data(), (long)b * band, (long)(n / 8 / nvv), (const double*)src, js.t2, nocc[sa], nva, nvb,
-                                         js.os != 0);
-                    }, ms2);
-                }
+        double* d_sums = (double*)c.alloc(2 * specs.size() * 8);
+        dev_zero(d_sums, 2 * specs.size() * 8, st);
+        StageTimer tm;     // the jobs without amplitudes; band_pipeline times the others
+        std::vector<std::vector<int>> pair_lists(specs.size());
+        for (size_t k = 0; k < specs.size(); k++) {
+            const JobSpec& js = specs[k];
+            if (js.npair == 0) continue;
+            const int sa = js.sa, sb = js.sb, nva = nvir[sa], nvb = nvir[sb];
+            const HalfPair &pa = sp.pr[sp.pr_of[sa]], &pb = sp.pr[sp.pr_of[sb]];
+            // pairs i-major (consecutive CTAs share L_i), tile pairs in row order
+            std::vector<int>& pl = pair_lists[k];
+            for (int i = 0; i < nocc[sa]; i++)
+                for (int j = 0; j < (js.os ? nocc[sb] : i + 1); j++) { pl.push_back(i); pl.push_back(j); }
+            std::vector<int> tl;
+            for (int A = 0; A < ntile(nva); A++)
+                for (int B = js.os ? 0 : A; B < ntile(nvb); B++) { tl.push_back(A); tl.push_back(B); }
+            int* d_pairs = (int*)c.alloc(pl.size() * 4);
+            int* d_tiles = (int*)c.alloc(tl.size() * 4);
+            h2d(d_pairs, pl.data(), pl.size() * 4, st);
+            h2d(d_tiles, tl.data(), tl.size() * 4, st);
+            double* d_part = (double*)c.alloc((size_t)js.npair * js.ntp * 2 * 8);
+            mp2k::Job jb{pa.L, pb.L, pa.nij, pb.nij, nva, nvb, nrow, d_eo[sa], d_eo[sb], d_ev[sa], d_ev[sb], d_pairs, d_tiles,
+                         (int)js.ntp, js.os, js.mode, nullptr, 0, d_part};
+            const mp2k::PartShare share{d_part, js.npair * js.ntp};
+            if (!js.t2) {
+                tm.mark(0, st);
+                mp2k::pair_launch(jb, 0, js.npair, st);
+                ao2mo::tree_sum(share, d_sums + 2 * k, st);
+                tm.mark(-1, st);
+            } else {
+                const long nvv = (long)nva * nvb, band = ao2mo_band_rows(d, js.npair, nvv * 8);
+                const int nbands = (int)((js.npair + band - 1) / band);
+                ao2mo::band_pipeline(d, st, nbands, (size_t)band * nvv * 8, [&](int b, double* buf) -> size_t {
+                    const long p0 = (long)b * band, p1 = std::min(js.npair, p0 + band);
+                    mp2k::Job jt = jb;
+                    jt.t2 = buf; jt.p0 = p0;
+                    mp2k::pair_launch(jt, p0, p1, st);
+                    if (b == nbands - 1) ao2mo::tree_sum(share, d_sums + 2 * k, st);
+                    return (size_t)(p1 - p0) * nvv * 8;
+                }, [&](int b, const void* src, size_t n) {
+                    mp2k::scatter_t2(pl.data(), (long)b * band, (long)(n / 8 / nvv), (const double*)src, js.t2, nocc[sa], nva, nvb,
+                                     js.os != 0);
+                }, ms2);
             }
-#ifndef B200JK_EMULATE
-            for (cudaEvent_t e : ev) cudaEventDestroy(e);
-#endif
-            std::vector<double> sums(2 * specs.size());
-            d2h(sums.data(), d_sums, sums.size() * 8, st);
-            dev_sync();
-            // the reference's combination: RMP2 dfmp2.py:109-119, UMP2 dfump2.py:119,154,164 (ex is stored with its sign)
-            if (nspin == 1) { e_out[0] = sums[0] + sums[1]; e_out[1] = sums[0]; }
-            else {
-                double ess = 0.0;
-                ess += (sums[0] + sums[1]) * 0.5;
-                ess += (sums[2] + sums[3]) * 0.5;
-                e_out[0] = ess; e_out[1] = sums[4];
-            }
-            d->mp2_ms[0] = ms1; d->mp2_ms[1] = ms2;
-        } catch (...) {
-            dev_sync();
-            for (void* p : owned) dev_free(p);
-            throw;
         }
+        std::vector<double> sums(2 * specs.size());
+        d2h(sums.data(), d_sums, sums.size() * 8, st);
         dev_sync();
-        for (void* p : owned) dev_free(p);
-        d->mp2_ms[2] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+        double ms_nt = 0.0;
+        tm.read(&ms_nt, nullptr, 1);
+        // the reference's combination: RMP2 dfmp2.py:109-119, UMP2 dfump2.py:119,154,164 (ex is stored with its sign)
+        if (nspin == 1) { e_out[0] = sums[0] + sums[1]; e_out[1] = sums[0]; }
+        else {
+            double ess = 0.0;
+            ess += (sums[0] + sums[1]) * 0.5;
+            ess += (sums[2] + sums[3]) * 0.5;
+            e_out[0] = ess; e_out[1] = sums[4];
+        }
+        d->mp2_ms[0] = ms1; d->mp2_ms[1] = ms2 + ms_nt;
+        d->mp2_ms[2] = c.finish();
     } catch (std::exception& e) { set_err(h, e.what()); return 2; }
     return 0;
 }
 
-extern "C" int b200jk_df_mp2_times(b200jk_handle h, double* ms, int n)
-{
-    if (!h || !h->df || !ms) { set_err(h, "call b200jk_df_build first"); return 1; }
-    for (int i = 0; i < n; i++) ms[i] = i < 3 ? h->df->mp2_ms[i] : 0.0;
-    return 0;
-}
+extern "C" int b200jk_df_mp2_times(b200jk_handle h, double* ms, int n) { return mo_times(h, &DFState::mp2_ms, ms, n); }

@@ -16,9 +16,7 @@
 // The emulation build runs the same CTA code on the host fragment model and factors with cpu_cholesky_lower.
 
 namespace rpak {
-using ao2mo::BM; using ao2mo::BN; using ao2mo::BK; using ao2mo::NT; using ao2mo::LDC; using ao2mo::PER_T;
-
-constexpr int RT = 256;     // threads of the diagonal sums
+using ao2mo::BM; using ao2mo::BN; using ao2mo::BK; using ao2mo::NT; using ao2mo::LDC; using ao2mo::PER_T; using ao2mo::RT;
 
 // L[r, k] over K = [spin 0 | spin 1]: L0 [naux][k1], L1 [naux][ld1]
 struct Seg {
@@ -41,8 +39,11 @@ typedef ao2mo::Gemm<SegA, SegB, NoSt> PiGemm;
 // every A element a thread stages in one k step has k = k0 + t % BK (MFAST = false), so one chi value per thread and k step;
 // it is loaded with the operands, one step ahead, and multiplied in at the put, after the MMAs that hide the loads
 static_assert(NT % BK == 0, "one k per thread in the A operand");
-AO_D double chi_at(const double* chi, long K, long k0, int t) { const long k = k0 + t % BK; return k < K ? chi[k] : 0.0; }
-AO_D void scale(double* ra, double cx) { for (int q = 0; q < PER_T; q++) ra[q] *= cx; }
+struct ChiHook {
+    const double* chi; long K; double cx;
+    AO_D void at(long k0, int t) { const long k = k0 + t % BK; cx = k < K ? chi[k] : 0.0; }
+    AO_D void apply(double* ra) const { for (int q = 0; q < PER_T; q++) ra[q] *= cx; }
+};
 
 struct Job {
     PiGemm g;           // M = N = naux, K = sum_s nocc_s nvir_s
@@ -74,57 +75,28 @@ AO_D void pi_epilogue(const Job& jb, const double* sm, long m0, long n0, int t)
     }
 }
 
-// thread t of the diagonal sums: its strided share of log L_PP (the factor's diagonal in M) and of Pi_PP
-AO_D void diag_share(const double* M, const double* dg, long N, int t, double* red)
-{
-    double a = 0.0, b = 0.0;
-    for (long P = t; P < N; P += RT) { a += log(M[P * N + P]); b += dg[P]; }
-    red[t] = a; red[RT + t] = b;
-}
-AO_D void red_step(double* red, int t, int s) { if (t < s) { red[t] += red[t + s]; red[RT + t] += red[RT + t + s]; } }
+// thread t of the diagonal sums: its strided share of 2 log L_PP (the factor's diagonal in M) and of Pi_PP
+struct DiagShare {
+    const double *M, *dg; long N;
+    AO_D void operator()(int t, double& a, double& b) const
+    {
+        for (long P = t; P < N; P += RT) { a += log(M[P * N + P]); b += dg[P]; }
+        a *= 2.0;
+    }
+};
 
 #ifndef B200JK_EMULATE
 __global__ void __launch_bounds__(NT) rpa_pi_kernel(Job jb)
 {
     __shared__ __align__(128) double sm[ao2mo::SMEM];
     const long m0 = (long)jb.tiles[2 * blockIdx.x] * BM, n0 = (long)jb.tiles[2 * blockIdx.x + 1] * BN;
-    const PiGemm& g = jb.g;
-    const int t = threadIdx.x, w = t >> 5;
+    const int t = threadIdx.x;
     ao2mo::fr::C c[4][4];
-#pragma unroll
-    for (int a = 0; a < 4; a++)
-#pragma unroll
-        for (int b = 0; b < 4; b++) ao2mo::fr::zero(c[a][b]);
-    double ra[PER_T], rb[PER_T];
-    ao2mo::fetch(g, m0, n0, 0, t, ra, rb);
-    double cx = chi_at(jb.chi, g.K, 0, t);
-    for (long k0 = 0; k0 < g.K; k0 += BK) {
-        scale(ra, cx);
-        ao2mo::put<PiGemm>(sm, t, ra, rb);
-        __syncthreads();
-        if (k0 + BK < g.K) {     // next k step in flight during the MMAs
-            ao2mo::fetch(g, m0, n0, k0 + BK, t, ra, rb);
-            cx = chi_at(jb.chi, g.K, k0 + BK, t);
-        }
-        ao2mo::warp_mma(sm, w, c);
-        __syncthreads();
-    }
-    ao2mo::warp_store(sm, w, c);
+    ChiHook hk{jb.chi, jb.g.K, 0.0};
+    ao2mo::k_loop(jb.g, m0, n0, 0, BK, jb.g.K, sm, t, hk, c);
+    ao2mo::warp_store(sm, t >> 5, c);
     __syncthreads();
     pi_epilogue(jb, sm, m0, n0, t);
-}
-
-__global__ void __launch_bounds__(RT) rpa_diag_kernel(const double* M, const double* dg, long N, double* out)
-{
-    __shared__ double red[2 * RT];
-    const int t = threadIdx.x;
-    diag_share(M, dg, N, t, red);
-    __syncthreads();
-    for (int s = RT / 2; s > 0; s >>= 1) {
-        red_step(red, t, s);
-        __syncthreads();
-    }
-    if (t == 0) { out[0] = 2.0 * red[0]; out[1] = red[RT]; }
 }
 
 static void pi_launch(const Job& jb, int ntile, cudaStream_t s)
@@ -132,50 +104,18 @@ static void pi_launch(const Job& jb, int ntile, cudaStream_t s)
     rpa_pi_kernel<<<ntile, NT, 0, s>>>(jb);
     CK(cudaGetLastError());
 }
-static void diag_launch(const double* M, const double* dg, long N, double* out, cudaStream_t s)
-{
-    rpa_diag_kernel<<<1, RT, 0, s>>>(M, dg, N, out);
-    CK(cudaGetLastError());
-}
 #else
-// the same CTA code, thread by thread and warp by warp, on the host model of the fragments
+// the same CTA code on the host model of the fragments
 static void pi_launch(const Job& jb, int ntile, stream_t)
 {
-    const PiGemm& g = jb.g;
-    std::vector<double> sm(ao2mo::SMEM), ra(NT * PER_T), rb(NT * PER_T), cx(NT);
-    std::vector<ao2mo::fr::C> cw(4 * 16);
-    typedef ao2mo::fr::C Acc[4][4];
-    Acc* c = reinterpret_cast<Acc*>(cw.data());
+    std::vector<double> sm(ao2mo::SMEM);
+    ao2mo::Acc c[4];
     for (int x = 0; x < ntile; x++) {
         const long m0 = (long)jb.tiles[2 * x] * BM, n0 = (long)jb.tiles[2 * x + 1] * BN;
-        for (ao2mo::fr::C& v : cw) ao2mo::fr::zero(v);
-        for (int t = 0; t < NT; t++) {
-            ao2mo::fetch(g, m0, n0, 0, t, &ra[t * PER_T], &rb[t * PER_T]);
-            cx[t] = chi_at(jb.chi, g.K, 0, t);
-        }
-        for (long k0 = 0; k0 < g.K; k0 += BK) {
-            for (int t = 0; t < NT; t++) {
-                scale(&ra[t * PER_T], cx[t]);
-                ao2mo::put<PiGemm>(sm.data(), t, &ra[t * PER_T], &rb[t * PER_T]);
-            }
-            if (k0 + BK < g.K)
-                for (int t = 0; t < NT; t++) {
-                    ao2mo::fetch(g, m0, n0, k0 + BK, t, &ra[t * PER_T], &rb[t * PER_T]);
-                    cx[t] = chi_at(jb.chi, g.K, k0 + BK, t);
-                }
-            for (int w = 0; w < 4; w++) ao2mo::warp_mma(sm.data(), w, c[w]);
-        }
+        ao2mo::k_loop(jb.g, m0, n0, 0, BK, jb.g.K, sm.data(), ChiHook{jb.chi, jb.g.K, 0.0}, c);
         for (int w = 0; w < 4; w++) ao2mo::warp_store(sm.data(), w, c[w]);
         for (int t = 0; t < NT; t++) pi_epilogue(jb, sm.data(), m0, n0, t);
     }
-}
-static void diag_launch(const double* M, const double* dg, long N, double* out, stream_t)
-{
-    std::vector<double> red(2 * RT);
-    for (int t = 0; t < RT; t++) diag_share(M, dg, N, t, red.data());
-    for (int s = RT / 2; s > 0; s >>= 1)
-        for (int t = 0; t < RT; t++) red_step(red.data(), t, s);
-    out[0] = 2.0 * red[0]; out[1] = red[RT];
 }
 #endif
 
@@ -187,39 +127,19 @@ extern "C" int b200jk_df_rpa(b200jk_handle h, int nspin, const double* const* c_
 {
     if (!h) return 1;
     try {
-        DFState* d = h->df;
-        if (!d || !d->d_cderi) throw std::runtime_error("call b200jk_df_build (or b200jk_df_set_cderi) before b200jk_df_rpa");
-        if (d->build_world != 1)
-            throw std::runtime_error("b200jk_df_rpa: a sharded tensor is not supported (Pi needs every auxiliary row of L)");
+        MoCall c(h, "b200jk_df_rpa", " (Pi needs every auxiliary row of L)");
+        DFState* d = c.d;
+        const stream_t st = c.st;
         if ((nspin != 1 && nspin != 2) || !c_occ || !nocc || !c_vir || !nvir || !e_ov || !f_ov || nw < 1 || !omega || !logdet ||
             !trace || (diel && nw != 1))
             throw std::runtime_error("bad arguments");
-        bool active[2] = {false, false};
-        for (int s = 0; s < nspin; s++) {
-            if (nocc[s] < 0 || nvir[s] < 0) throw std::runtime_error("bad arguments: negative orbital count");
-            active[s] = nocc[s] > 0 && nvir[s] > 0;
-            if (active[s] && (!c_occ[s] || !c_vir[s] || !e_ov[s] || !f_ov[s])) throw std::runtime_error("bad arguments");
-        }
-        auto t_start = std::chrono::steady_clock::now();
+        // the active spins in spin order: the K segments of Pi
+        ActiveSpins sp(nspin, c_occ, nocc, c_vir, nvir, e_ov, f_ov);
         const int nao = h->nsph, nrow = d->nrow;
         const long N = nrow;
-#ifndef B200JK_EMULATE
-        CK(cudaSetDevice(h->device));
-        cudaStream_t st = h->stream;
-#else
-        stream_t st = 0;
-#endif
-        // stage-1 pairs (co, cv) of the active spins, in spin order: the K segments of Pi
-        HalfPair pr[2];
-        int npr = 0, na_max = 1;
         long K = 0;
-        for (int s = 0; s < nspin; s++)
-            if (active[s]) {
-                pr[npr] = HalfPair{{c_occ[s], c_vir[s]}, {nocc[s], nvir[s]}, 0, (long)nocc[s] * nvir[s], nullptr, {nullptr, nullptr}};
-                na_max = std::max(na_max, std::min(nocc[s], nvir[s]));
-                K += pr[npr++].nij;
-            }
-        const int rb = half_block_rows(nrow, nao, na_max);
+        for (int q = 0; q < sp.npr; q++) K += sp.pr[q].nij;
+        const int rb = half_block_rows(nrow, nao, sp.na_max);
 #ifndef B200JK_EMULATE
         int lwork = 0;
         CKS(cusolverDnSetStream(d->cusolver, st));
@@ -228,131 +148,89 @@ extern "C" int b200jk_df_rpa(b200jk_handle h, int nspin, const double* const* c_
 #else
         const int lwork = 0;
 #endif
-        double need = (double)rb * nao * na_max + (double)N * N * (diel ? 2 : 1) + lwork + 3.0 * K + N + 2.0 * nw;
-        for (int q = 0; q < npr; q++) need += (double)nrow * pr[q].nij;
+        double need = (double)rb * nao * sp.na_max + (double)N * N * (diel ? 2 : 1) + lwork + 3.0 * K + N + 2.0 * nw;
+        for (int q = 0; q < sp.npr; q++) need += (double)nrow * sp.pr[q].nij;
         ao2mo_check_fit(8.0 * need, "DF-RPA: the half-transformed integrals L[naux, nocc nvir] of each spin, Pi[naux, naux] and "
                                     "the factorisation workspace");
 
-        std::vector<void*> owned;
-        auto alloc = [&](size_t bytes) { void* p = dev_alloc(bytes); owned.push_back(p); return p; };
-        try {
-            double ms1 = 0.0, ms2 = 0.0, ms3 = 0.0;
-            if (npr > 0) {
-                for (int q = 0; q < npr; q++) {
-                    pr[q].L = (double*)alloc((size_t)std::max(nrow, 1) * pr[q].nij * 8);
-                    for (int s = 0; s < 2; s++) {
-                        pr[q].dc[s] = (double*)alloc((size_t)nao * pr[q].n[s] * 8);
-                        h2d(pr[q].dc[s], pr[q].c[s], (size_t)nao * pr[q].n[s] * 8, st);
-                    }
-                }
-                double* d_Y = (double*)dev_alloc((size_t)rb * nao * na_max * 8);
-                try { ms1 = half_transform(d, nao, st, pr, npr, d_Y, rb); } catch (...) { dev_sync(); dev_free(d_Y); throw; }
-                dev_sync();
-                dev_free(d_Y);
+        const double ms1 = half_transform(c, nao, sp.pr, sp.npr, rb, sp.na_max);
+        // e_ov, f_ov of the active spins as one K vector, in the order of the segments
+        double* d_e = (double*)c.alloc((size_t)std::max(K, 1L) * 8);
+        double* d_f = (double*)c.alloc((size_t)std::max(K, 1L) * 8);
+        double* d_chi = (double*)c.alloc((size_t)std::max(K, 1L) * 8);
+        for (int s = 0; s < nspin; s++)
+            if (sp.active(s)) {
+                const int q = sp.pr_of[s];
+                const long k0 = q ? sp.pr[0].nij : 0;
+                h2d(d_e + k0, e_ov[s], (size_t)sp.pr[q].nij * 8, st);
+                h2d(d_f + k0, f_ov[s], (size_t)sp.pr[q].nij * 8, st);
             }
-            // e_ov, f_ov of the active spins as one K vector, in the order of the segments
-            double* d_e = (double*)alloc((size_t)std::max(K, 1L) * 8);
-            double* d_f = (double*)alloc((size_t)std::max(K, 1L) * 8);
-            double* d_chi = (double*)alloc((size_t)std::max(K, 1L) * 8);
-            for (int s = 0, q = 0; s < nspin; s++)
-                if (active[s]) {
-                    const long k0 = q ? pr[0].nij : 0;
-                    h2d(d_e + k0, e_ov[s], (size_t)pr[q].nij * 8, st);
-                    h2d(d_f + k0, f_ov[s], (size_t)pr[q].nij * 8, st);
-                    q++;
-                }
-            double* d_M = (double*)alloc((size_t)N * N * 8);
-            double* d_dg = (double*)alloc((size_t)N * 8);
-            double* d_diel = diel ? (double*)alloc((size_t)N * N * 8) : nullptr;
-            double* d_out = (double*)alloc((size_t)2 * nw * 8);
-            int* d_info = (int*)alloc((size_t)nw * 4);
-            dev_zero(d_info, (size_t)nw * 4, st);
+        double* d_M = (double*)c.alloc((size_t)N * N * 8);
+        double* d_dg = (double*)c.alloc((size_t)N * 8);
+        double* d_diel = diel ? (double*)c.alloc((size_t)N * N * 8) : nullptr;
+        double* d_out = (double*)c.alloc((size_t)2 * nw * 8);
+        int* d_info = (int*)c.alloc((size_t)nw * 4);
+        dev_zero(d_info, (size_t)nw * 4, st);
+        const long nt = (N + ao2mo::BM - 1) / ao2mo::BM;
+        std::vector<int> tl;
+        for (int A = 0; A < nt; A++)
+            for (int B = A; B < nt; B++) { tl.push_back(A); tl.push_back(B); }
+        const int ntile = (int)(tl.size() / 2);
+        int* d_tiles = (int*)c.alloc(tl.size() * 4);
+        h2d(d_tiles, tl.data(), tl.size() * 4, st);
+        const long k1 = sp.npr > 0 ? sp.pr[0].nij : 0, ld1 = sp.npr > 1 ? sp.pr[1].nij : 0;
+        const double* L0 = sp.npr > 0 ? sp.pr[0].L : nullptr;
+        const double* L1 = sp.npr > 1 ? sp.pr[1].L : nullptr;
+        const rpak::Seg seg{L0, L1, k1, ld1};
+        rpak::Job jb{rpak::PiGemm{N, N, K, {seg}, {seg}, {}, 0, 0, 0}, d_chi, d_tiles, d_M, d_dg, d_diel};
+        // M = L L^T in place (d_info[w] != 0: not positive definite)
 #ifndef B200JK_EMULATE
-            double* d_work = (double*)alloc((size_t)std::max(lwork, 1) * 8);
-#endif
-            const long nt = (N + ao2mo::BM - 1) / ao2mo::BM;
-            std::vector<int> tl;
-            for (int A = 0; A < nt; A++)
-                for (int B = A; B < nt; B++) { tl.push_back(A); tl.push_back(B); }
-            const int ntile = (int)(tl.size() / 2);
-            int* d_tiles = (int*)alloc(tl.size() * 4);
-            h2d(d_tiles, tl.data(), tl.size() * 4, st);
-            const long k1 = npr > 0 ? pr[0].nij : 0, ld1 = npr > 1 ? pr[1].nij : 0;
-            const double* L0 = npr > 0 ? pr[0].L : nullptr;
-            const double* L1 = npr > 1 ? pr[1].L : nullptr;
-            const rpak::Seg seg{L0, L1, k1, ld1};
-            rpak::Job jb{rpak::PiGemm{N, N, K, {seg}, {seg}, {}, 0, 0, 0}, d_chi, d_tiles, d_M, d_dg, d_diel};
-#ifndef B200JK_EMULATE
-            std::vector<cudaEvent_t> ev(3 * (size_t)nw, nullptr);
-            for (cudaEvent_t& e : ev) CK(cudaEventCreate(&e));
-            try {
-                for (int w = 0; w < nw; w++) {
-                    CK(cudaEventRecord(ev[3 * w], st));
-                    launch_1d(K, rpak::ChiFn{d_e, d_f, omega[w] * omega[w], d_chi}, st);
-                    rpak::pi_launch(jb, ntile, st);
-                    CK(cudaEventRecord(ev[3 * w + 1], st));
-                    CKS(cusolverDnDpotrf(d->cusolver, CUBLAS_FILL_MODE_LOWER, (int)N, d_M, (int)N, d_work, lwork, d_info + w));
-                    rpak::diag_launch(d_M, d_dg, N, d_out + 2 * w, st);
-                    CK(cudaEventRecord(ev[3 * w + 2], st));
-                }
-                CK(cudaStreamSynchronize(st));
-                for (int w = 0; w < nw; w++) {
-                    float t = 0;
-                    CK(cudaEventElapsedTime(&t, ev[3 * w], ev[3 * w + 1]));
-                    ms2 += t;
-                    CK(cudaEventElapsedTime(&t, ev[3 * w + 1], ev[3 * w + 2]));
-                    ms3 += t;
-                }
-            } catch (...) {
-                for (cudaEvent_t e : ev) cudaEventDestroy(e);
-                throw;
-            }
-            for (cudaEvent_t e : ev) cudaEventDestroy(e);
+        double* d_work = (double*)c.alloc((size_t)std::max(lwork, 1) * 8);
+        auto factor = [&](int w) {
+            CKS(cusolverDnDpotrf(d->cusolver, CUBLAS_FILL_MODE_LOWER, (int)N, d_M, (int)N, d_work, lwork, d_info + w));
+        };
 #else
-            std::vector<double> a((size_t)N * N);
-            for (int w = 0; w < nw; w++) {
-                launch_1d(K, rpak::ChiFn{d_e, d_f, omega[w] * omega[w], d_chi}, st);
-                rpak::pi_launch(jb, ntile, st);
-                // cpu_cholesky_lower reads the row-major lower triangle: mirror the upper one that the epilogue wrote
-                for (long m = 0; m < N; m++)
-                    for (long n = 0; n < N; n++) a[m * N + n] = d_M[std::min(m, n) * N + std::max(m, n)];
-                bool ok = true;
-                cpu_cholesky_lower(a, (int)N, ok);
-                if (!ok) { d_info[w] = 1; continue; }
-                for (long P = 0; P < N; P++) d_M[P * N + P] = a[P * N + P];
-                rpak::diag_launch(d_M, d_dg, N, d_out + 2 * w, st);
-            }
+        std::vector<double> a((size_t)N * N);
+        auto factor = [&](int w) {
+            // cpu_cholesky_lower reads the row-major lower triangle: mirror the upper one that the epilogue wrote
+            for (long m = 0; m < N; m++)
+                for (long n = 0; n < N; n++) a[m * N + n] = d_M[std::min(m, n) * N + std::max(m, n)];
+            bool ok = true;
+            cpu_cholesky_lower(a, (int)N, ok);
+            if (!ok) { d_info[w] = 1; return; }
+            for (long P = 0; P < N; P++) d_M[P * N + P] = a[P * N + P];
+        };
 #endif
-            std::vector<int> info(nw);
-            std::vector<double> out((size_t)2 * nw);
-            d2h(info.data(), d_info, (size_t)nw * 4, st);
-            d2h(out.data(), d_out, out.size() * 8, st);
-            if (diel) d2h(diel, d_diel, (size_t)N * N * 8, st);
-            dev_sync();
-            for (int w = 0; w < nw; w++) {
-                if (info[w] == 0) continue;
-                char buf[400];
-                snprintf(buf, sizeof buf, "DF-RPA: I - Pi(omega) is not positive definite at omega = %.10g (potrf info %d); RPA is not "
-                         "well-defined for degenerate systems or for occupied orbitals above virtual ones", omega[w], info[w]);
-                throw std::runtime_error(buf);
-            }
-            for (int w = 0; w < nw; w++) { logdet[w] = out[2 * w]; trace[w] = out[2 * w + 1]; }
-            d->rpa_ms[0] = ms1; d->rpa_ms[1] = ms2; d->rpa_ms[2] = ms3;
-        } catch (...) {
-            dev_sync();
-            for (void* p : owned) dev_free(p);
-            throw;
+        StageTimer tm;     // [0] chi and Pi, [1] factorisation and diagonal sums
+        for (int w = 0; w < nw; w++) {
+            tm.mark(0, st);
+            launch_1d(K, rpak::ChiFn{d_e, d_f, omega[w] * omega[w], d_chi}, st);
+            rpak::pi_launch(jb, ntile, st);
+            tm.mark(1, st);
+            factor(w);
+            ao2mo::tree_sum(rpak::DiagShare{d_M, d_dg, N}, d_out + 2 * w, st);
+            tm.mark(-1, st);
         }
+        std::vector<int> info(nw);
+        std::vector<double> out((size_t)2 * nw);
+        d2h(info.data(), d_info, (size_t)nw * 4, st);
+        d2h(out.data(), d_out, out.size() * 8, st);
+        if (diel) d2h(diel, d_diel, (size_t)N * N * 8, st);
         dev_sync();
-        for (void* p : owned) dev_free(p);
-        d->rpa_ms[3] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+        for (int w = 0; w < nw; w++) {
+            if (info[w] == 0) continue;
+            char buf[400];
+            snprintf(buf, sizeof buf, "DF-RPA: I - Pi(omega) is not positive definite at omega = %.10g (potrf info %d); RPA is not "
+                     "well-defined for degenerate systems or for occupied orbitals above virtual ones", omega[w], info[w]);
+            throw std::runtime_error(buf);
+        }
+        for (int w = 0; w < nw; w++) { logdet[w] = out[2 * w]; trace[w] = out[2 * w + 1]; }
+        double ms23[2];
+        tm.read(ms23, nullptr, 2);
+        d->rpa_ms[0] = ms1; d->rpa_ms[1] = ms23[0]; d->rpa_ms[2] = ms23[1];
+        d->rpa_ms[3] = c.finish();
     } catch (std::exception& e) { set_err(h, e.what()); return 2; }
     return 0;
 }
 
-extern "C" int b200jk_df_rpa_times(b200jk_handle h, double* ms, int n)
-{
-    if (!h || !h->df || !ms) { set_err(h, "call b200jk_df_build first"); return 1; }
-    for (int i = 0; i < n; i++) ms[i] = i < 4 ? h->df->rpa_ms[i] : 0.0;
-    return 0;
-}
+extern "C" int b200jk_df_rpa_times(b200jk_handle h, double* ms, int n) { return mo_times(h, &DFState::rpa_ms, ms, n); }

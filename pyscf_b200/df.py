@@ -50,6 +50,72 @@ def _iden_coeffs(mo1, mo2):
     return a.shape == b.shape and bool(a.size == 0 or abs(a - b).max() < 1e-13)
 
 
+# ---- shared by the MO consumers of the tensor (DF.ao2mo, pyscf_b200.dfmp2, pyscf_b200.rpa) ------------------------------------
+
+def _check_df(with_df, method, why):
+    """nao of a built, unsharded with_df; method names the caller in the message, why says what sharding would break."""
+    if with_df.shard is not None:
+        raise NotImplementedError('%s on a sharded tensor (DF(shard=...)) is not implemented: %s' % (method, why))
+    with_df.get_naoaux()
+    return with_df.nao
+
+
+def _coeff(c, nao, what, method):
+    """c as a contiguous float64 [nao, n] array; complex coefficients and a wrong nao are refused."""
+    a = np.asarray(c)
+    if np.iscomplexobj(a):
+        raise NotImplementedError('%s: complex MO coefficients are not supported' % method)
+    if a.ndim != 2 or a.shape[0] != nao:
+        raise ValueError('%s: %s coefficients must be [nao, n] with nao = %d, got shape %s' % (method, what, nao, a.shape))
+    return np.ascontiguousarray(a, dtype=np.float64)
+
+
+class _ERIS:
+    """What DF-MP2 and DF-RPA need of DFMP2.ao2mo's result (_make_df_eris, pyscf/mp/dfmp2.py:215-272): the active coefficients,
+    nocc, nvir, naux.  L[P, ia] stays on the device, so its blocks cannot be read."""
+
+    dtype = np.float64
+
+    def __init__(self, with_df, occ_coeff, vir_coeff, unrestricted, who):
+        self.with_df = with_df
+        self.occ_coeff, self.vir_coeff = occ_coeff, vir_coeff
+        self.unrestricted = unrestricted
+        self.naux = with_df.get_naoaux()
+        if unrestricted:
+            self.nocc = tuple(c.shape[1] for c in occ_coeff)
+            self.nvir = tuple(c.shape[1] for c in vir_coeff)
+        else:
+            self.nocc, self.nvir = occ_coeff.shape[1], vir_coeff.shape[1]
+        self._who = who
+
+    def get_ov_blk(self, *args):
+        raise NotImplementedError('%s keeps L[P, ia] on the device; get_ov_blk is not available' % self._who)
+
+    def get_occ_blk(self, *args):
+        raise NotImplementedError('%s keeps L[P, ia] on the device; get_occ_blk is not available' % self._who)
+
+
+def _eris_ao2mo(obj, who):
+    """The ao2mo(mo_coeff, ovL, ovL_to_save) that patch() puts on a DFMP2 / RPA instance obj: the active orbitals of
+    obj.split_mo_coeff() as an _ERIS."""
+    def ao2mo(mo_coeff=None, ovL=None, ovL_to_save=None):
+        if ovL is not None or ovL_to_save is not None:
+            raise NotImplementedError('%s keeps the ovL integrals on the device; ovL / ovL_to_save are not supported' % who)
+        sp = obj.split_mo_coeff()
+        if len(sp) == 2:
+            return _ERIS(obj.with_df, tuple(s[1] for s in sp), tuple(s[2] for s in sp), True, who)
+        return _ERIS(obj.with_df, sp[1], sp[2], False, who)
+    return ao2mo
+
+
+def _times(with_df, fn, keys):
+    """{key: ms} of the last call, from the C function fn (b200jk_df_*_times)."""
+    h = with_df._handle
+    ms = np.zeros(len(keys))
+    h.check(getattr(h.lib, fn)(h._h, _lib.dptr(ms), len(keys)), fn)
+    return dict(zip(keys, ms.tolist()))
+
+
 class DF:
     def __init__(self, mol, auxbasis=None, device=0, libpath=None, shard=None, pair_tol=None):
         self.mol = mol
@@ -376,18 +442,11 @@ class DF:
         if len(mo_coeffs) != 4:
             raise ValueError('DF.ao2mo needs one [nao, n] array or four of them, got %d' % len(mo_coeffs))
         self.get_naoaux()
-        nao = self.nao
-        cs = []
-        for c in mo_coeffs:
-            a = np.asarray(c)
-            if np.iscomplexobj(a):
-                raise NotImplementedError('DF.ao2mo: complex MO coefficients are not supported')
-            if a.ndim != 2 or a.shape[0] != nao:
-                raise ValueError('DF.ao2mo: MO coefficients must be [nao, n] with nao = %d, got shape %s' % (nao, a.shape))
-            cs.append(a)
-        # _conc_mos (pyscf/ao2mo/incore.py:244-262): s2 only for identical double-precision sets
-        s12 = bool(compact) and np.result_type(cs[0], cs[1]) == np.double and _iden_coeffs(mo_coeffs[0], mo_coeffs[1])
-        s34 = bool(compact) and np.result_type(cs[2], cs[3]) == np.double and _iden_coeffs(mo_coeffs[2], mo_coeffs[3])
+        mo_coeffs = [np.asarray(c) for c in mo_coeffs]
+        cs = [_coeff(c, self.nao, 'MO', 'DF.ao2mo') for c in mo_coeffs]
+        # _conc_mos (pyscf/ao2mo/incore.py:244-262): s2 only for identical sets given in double precision
+        s12 = bool(compact) and np.result_type(*mo_coeffs[:2]) == np.double and _iden_coeffs(mo_coeffs[0], mo_coeffs[1])
+        s34 = bool(compact) and np.result_type(*mo_coeffs[2:]) == np.double and _iden_coeffs(mo_coeffs[2], mo_coeffs[3])
         sym = s12 == s34 and _iden_coeffs(mo_coeffs[0], mo_coeffs[2]) and _iden_coeffs(mo_coeffs[1], mo_coeffs[3])
         n = [a.shape[1] for a in cs]
         nij = n[0] * (n[0] + 1) // 2 if s12 else n[0] * n[1]
@@ -395,7 +454,6 @@ class DF:
         out = np.empty((nij, nkl))
         if out.size == 0:
             return out
-        cs = [np.ascontiguousarray(a, dtype=np.float64) for a in cs]
         h = self._handle
         if sym:
             h.check(h.lib.b200jk_df_ao2mo(h._h, _lib.dptr(cs[0]), n[0], _lib.dptr(cs[1]), n[1], int(s12), None, 0, None, 0, 0,
@@ -422,10 +480,7 @@ class DF:
     def ao2mo_times(self):
         """Milliseconds of the last ao2mo / get_eri: {'stage1', 'stage2'} device time of the half transforms and of the
         output GEMMs (CUDA events), 'total' host time of the whole call including the copies to the caller."""
-        h = self._handle
-        ms = np.zeros(3)
-        h.check(h.lib.b200jk_df_ao2mo_times(h._h, _lib.dptr(ms), 3), 'b200jk_df_ao2mo_times')
-        return {'stage1': float(ms[0]), 'stage2': float(ms[1]), 'total': float(ms[2])}
+        return _times(self, 'b200jk_df_ao2mo_times', ('stage1', 'stage2', 'total'))
 
     def stats(self):
         return self._handle.stats()

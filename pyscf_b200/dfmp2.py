@@ -13,6 +13,7 @@ This module does not import pyscf: patch() only replaces two methods of the inst
 import numpy as np
 
 from . import lib as _lib
+from .df import _check_df, _coeff, _eris_ao2mo, _times
 
 _T2_MEMORY_MSG = 'Insufficient memory for holding t2 incore. Please rerun with `with_t2 = False`.'   # dfmp2.py:59-61
 
@@ -27,23 +28,6 @@ class TaggedFloat(float):
         return x
 
 
-def _check_df(with_df, method='DF-MP2', why='the pair energies are not linear in the local rows'):
-    """nao of a built, unsharded with_df (shared with pyscf_b200.rpa, which passes its own method name and reason)."""
-    if with_df.shard is not None:
-        raise NotImplementedError('%s on a sharded tensor (DF(shard=...)) is not implemented: %s' % (method, why))
-    with_df.get_naoaux()
-    return with_df.nao
-
-
-def _coeff(c, nao, what, method='DF-MP2'):
-    a = np.asarray(c)
-    if np.iscomplexobj(a):
-        raise NotImplementedError('%s: complex MO coefficients are not supported' % method)
-    if a.ndim != 2 or a.shape[0] != nao:
-        raise ValueError('%s: %s coefficients must be [nao, n] with nao = %d, got shape %s' % (method, what, nao, a.shape))
-    return np.ascontiguousarray(a, dtype=np.float64)
-
-
 def _energy(e, n, what):
     e = np.ascontiguousarray(np.asarray(e, dtype=np.float64).ravel())
     if len(e) != n:
@@ -53,10 +37,10 @@ def _energy(e, n, what):
 
 def _run(with_df, cos, cvs, eos, evs, t2_shapes):
     """b200jk_df_mp2 over nspin = len(cos) spins; t2_shapes: None or the shapes of the amplitude blocks to return."""
-    nao = _check_df(with_df)
+    nao = _check_df(with_df, 'DF-MP2', 'the pair energies are not linear in the local rows')
     ns = len(cos)
-    cos = [_coeff(c, nao, 'occupied') for c in cos]
-    cvs = [_coeff(c, nao, 'virtual') for c in cvs]
+    cos = [_coeff(c, nao, 'occupied', 'DF-MP2') for c in cos]
+    cvs = [_coeff(c, nao, 'virtual', 'DF-MP2') for c in cvs]
     nocc = np.array([c.shape[1] for c in cos], dtype=np.int32)
     nvir = np.array([c.shape[1] for c in cvs], dtype=np.int32)
     eos = [_energy(e, n, 'occupied') for e, n in zip(eos, nocc)]
@@ -89,34 +73,10 @@ def ukernel(with_df, occ_coeffs, vir_coeffs, occ_energies, vir_energies, with_t2
     return _run(with_df, list(occ_coeffs), list(vir_coeffs), list(occ_energies), list(vir_energies), shapes if with_t2 else None)
 
 
-class _ERIS:
-    """What the kernels need of _make_df_eris's result (dfmp2.py:215-272): the active coefficients, nocc, nvir, naux."""
-
-    def __init__(self, with_df, occ_coeff, vir_coeff, unrestricted):
-        self.with_df = with_df
-        self.occ_coeff, self.vir_coeff = occ_coeff, vir_coeff
-        self.unrestricted = unrestricted
-        self.naux = with_df.get_naoaux()
-        if unrestricted:
-            self.nocc = tuple(c.shape[1] for c in occ_coeff)
-            self.nvir = tuple(c.shape[1] for c in vir_coeff)
-        else:
-            self.nocc, self.nvir = occ_coeff.shape[1], vir_coeff.shape[1]
-
-
 def patch(pt):
     """Route a PySCF DFRMP2 / DFUMP2 instance whose with_df is a pyscf_b200.df.DF through the GPU kernels: pt.ao2mo and
     pt.init_amps are replaced on the instance, everything else (get_mo_energy, e_hf, frozen orbitals through split_mo_coeff /
     split_mo_energy, SCS, make_rdm1 on the returned t2, _finalize) stays PySCF's.  Returns pt."""
-    def ao2mo(mo_coeff=None, ovL=None, ovL_to_save=None):
-        if ovL is not None or ovL_to_save is not None:
-            raise NotImplementedError('DF-MP2 on the GPU keeps the ovL integrals on the device; ovL / ovL_to_save are not supported')
-        sp = pt.split_mo_coeff()
-        unrestricted = len(sp) == 2
-        if unrestricted:
-            return _ERIS(pt.with_df, tuple(s[1] for s in sp), tuple(s[2] for s in sp), True)
-        return _ERIS(pt.with_df, sp[1], sp[2], False)
-
     def init_amps(mo_energy=None, mo_coeff=None, eris=None, with_t2=True):
         if eris is None:
             eris = pt.ao2mo(mo_coeff)
@@ -133,7 +93,7 @@ def patch(pt):
             return ukernel(eris.with_df, eris.occ_coeff, eris.vir_coeff, [s[1] for s in se], [s[2] for s in se], with_t2)
         return kernel(eris.with_df, eris.occ_coeff, eris.vir_coeff, se[1], se[2], with_t2)
 
-    pt.ao2mo = ao2mo
+    pt.ao2mo = _eris_ao2mo(pt, 'DF-MP2 on the GPU')
     pt.init_amps = init_amps
     return pt
 
@@ -141,7 +101,4 @@ def patch(pt):
 def times(with_df):
     """Milliseconds of the last DF-MP2 call: {'stage1', 'stage2'} device time of the half transform and of the pair kernel
     (CUDA events), 'total' host time of the whole call."""
-    h = with_df._handle
-    ms = np.zeros(3)
-    h.check(h.lib.b200jk_df_mp2_times(h._h, _lib.dptr(ms), 3), 'b200jk_df_mp2_times')
-    return {'stage1': float(ms[0]), 'stage2': float(ms[1]), 'total': float(ms[2])}
+    return _times(with_df, 'b200jk_df_mp2_times', ('stage1', 'stage2', 'total'))

@@ -17,7 +17,7 @@ import pyscf: patch() only replaces three methods of the instance it is given.
 import numpy as np
 
 from . import lib as _lib
-from .dfmp2 import _check_df, _coeff
+from .df import DF, _check_df, _coeff, _eris_ao2mo, _times
 
 _METHOD = 'DF-RPA'
 
@@ -99,48 +99,15 @@ def dielectric_matrix(with_df, occ_coeffs, vir_coeffs, e_ovs, f_ovs, omega):
     return _run(with_df, occ_coeffs, vir_coeffs, e_ovs, f_ovs, [float(omega)], True)[2]
 
 
-class _ERIS:
-    """What the kernels need of DFMP2.ao2mo's result (_make_df_eris, pyscf/mp/dfmp2.py:215-272): the active coefficients,
-    nocc, nvir, naux.  L[P, ia] stays on the device, so its blocks cannot be read."""
-
-    dtype = np.float64
-
-    def __init__(self, with_df, occ_coeff, vir_coeff, unrestricted):
-        self.with_df = with_df
-        self.occ_coeff, self.vir_coeff = occ_coeff, vir_coeff
-        self.unrestricted = unrestricted
-        self.naux = with_df.get_naoaux()
-        if unrestricted:
-            self.nocc = tuple(c.shape[1] for c in occ_coeff)
-            self.nvir = tuple(c.shape[1] for c in vir_coeff)
-        else:
-            self.nocc, self.nvir = occ_coeff.shape[1], vir_coeff.shape[1]
-
-    def get_ov_blk(self, *args):
-        raise NotImplementedError('%s keeps L[P, ia] on the device; get_ov_blk is not available' % _METHOD)
-
-    def get_occ_blk(self, *args):
-        raise NotImplementedError('%s keeps L[P, ia] on the device; get_occ_blk is not available' % _METHOD)
-
-
 def patch(rpa):
     """Route a PySCF RPA / URPA instance whose with_df is a pyscf_b200.df.DF through the GPU kernels: rpa.ao2mo,
     rpa.make_dielectric_matrix and rpa.kernel are replaced on the instance.  kernel keeps the reference's sequence (rpa.py:188-210):
     the complex-orbital NotImplementedError, dump_flags, get_e_hf, make_e_ov / make_f_ov (frozen orbitals and the small-gap
     warning stay PySCF's), then e_hf, e_corr and _finalize.  RPA(mf) on an unfitted mf makes a CPU df.DF: set rpa.with_df to a
     pyscf_b200.df.DF first.  Returns rpa."""
-    from .df import DF
     if not isinstance(getattr(rpa, 'with_df', None), DF):
         raise TypeError('%s: rpa.with_df must be a pyscf_b200.df.DF (got %s); set rpa.with_df = pyscf_b200.df.DF(mol, auxbasis)'
                         '.build() before patch()' % (_METHOD, type(getattr(rpa, 'with_df', None)).__name__))
-
-    def ao2mo(mo_coeff=None, ovL=None, ovL_to_save=None):
-        if ovL is not None or ovL_to_save is not None:
-            raise NotImplementedError('%s keeps the ovL integrals on the device; ovL / ovL_to_save are not supported' % _METHOD)
-        sp = rpa.split_mo_coeff()
-        if len(sp) == 2:
-            return _ERIS(rpa.with_df, tuple(s[1] for s in sp), tuple(s[2] for s in sp), True)
-        return _ERIS(rpa.with_df, sp[1], sp[2], False)
 
     def make_dielectric_matrix(omega, e_ov=None, f_ov=None, eris=None, max_memory=None, blksize=None):
         if e_ov is None:
@@ -165,7 +132,7 @@ def patch(rpa):
         rpa._finalize()
         return rpa.e_corr
 
-    rpa.ao2mo = ao2mo
+    rpa.ao2mo = _eris_ao2mo(rpa, _METHOD)
     rpa.make_dielectric_matrix = make_dielectric_matrix
     rpa.kernel = kernel_
     return rpa
@@ -174,7 +141,4 @@ def patch(rpa):
 def times(with_df):
     """Milliseconds of the last RPA call: {'stage1', 'pi', 'factor'} device time of the half transform, of the Pi GEMMs and of
     the factorisations (CUDA events, summed over the frequencies), 'total' host time of the whole call."""
-    h = with_df._handle
-    ms = np.zeros(4)
-    h.check(h.lib.b200jk_df_rpa_times(h._h, _lib.dptr(ms), 4), 'b200jk_df_rpa_times')
-    return {'stage1': float(ms[0]), 'pi': float(ms[1]), 'factor': float(ms[2]), 'total': float(ms[3])}
+    return _times(with_df, 'b200jk_df_rpa_times', ('stage1', 'pi', 'factor', 'total'))
