@@ -60,6 +60,16 @@ constexpr bool class_prefers_ppw(int li, int lj, int lk, int ll)
     return (li == 2 && lj == 2 && lk == 1 && ll == 1) || (li == 3 && lj == 3 && lk == 2 && ll == 0) || (li == 3 && lj == 2 && lk == 2 && ll == 0) ||
            (li == 2 && lj == 2 && lk == 2 && ll == 1) || (li == 2 && lj == 2 && lk == 2 && ll == 0) || (li == 3 && lj == 2 && lk == 1 && ll == 1);
 }
+// Classes whose phase E stays one reduction per lane and sum (phase_digest_lane) instead of one per distinct element through
+// the slot's scratch (DigestCfg): the five where the scratch rounds, each behind two barriers of a multi-warp group, cost more
+// than the reductions they save.  Class times on one H100 80GB HBM3 at 700 W, benzene/cc-pVTZ, classes serialised, best of 3,
+// per-lane -> per-element (ms): (fd|dd) 0.763 -> 0.848, (fs|dd) 0.601 -> 0.647, (dd|dp) 1.317 -> 1.355, (fd|fd) 0.463 -> 0.484,
+// (dd|dd) 0.390 -> 0.406; the old library's own runs differ by up to 0.02 ms.
+constexpr bool class_reduces_per_lane(int li, int lj, int lk, int ll)
+{
+    return (li == 3 && lj == 2 && lk == 2 && ll == 2) || (li == 3 && lj == 0 && lk == 2 && ll == 2) || (li == 2 && lj == 2 && lk == 2 && ll == 1) ||
+           (li == 3 && lj == 2 && lk == 3 && ll == 2) || (li == 2 && lj == 2 && lk == 2 && ll == 2);
+}
 template <class C>
 struct GroupCfg {
     static constexpr int G = C::G;
@@ -102,6 +112,7 @@ template <class C>
 struct LaneCtx {
     ThreadCtx<C> t;
     double jij[C::NV];
+    double jkl;      // phase E: this lane's J[kl] sum of the current density (digest_j)
     int grp, lt, slot, valid;
     int ibp, ikp;
     int sr;          // omega < 0 only: 0 = Coulomb pass, 1 = (negated) erf pass of the current primitive quartet
@@ -317,17 +328,58 @@ void group_proc(const KParams& P, BlockSmem<C>& sm, int grp, int nk, int bx,
         }
         }
         // ---- phase E: digestion
-        B2_GROUP_LANES(lt)
-            LaneCtx<C>& L = B2_CTX(tid0 + lt);
-            if (L.valid) {
-                SlotSmem<C>& s = sm.slot[L.slot];
-                if (s.active) {
-                    if (P.vj) phase_digest<C>(s, L.t, sm.bra.i0, sm.bra.j0, P.n, P.n_dm_j, P.dmj, nullptr, P.vj, nullptr,
-                                              P.n_dm_j == 1 ? L.jij : nullptr);
-                    if (P.vk) phase_digest<C>(s, L.t, sm.bra.i0, sm.bra.j0, P.n, P.n_dm_k, nullptr, P.dmk, nullptr, P.vk, nullptr);
+        if constexpr (class_reduces_per_lane(C::LI, C::LJ, C::LK, C::LL)) {
+            B2_GROUP_LANES(lt)
+                LaneCtx<C>& L = B2_CTX(tid0 + lt);
+                if (L.valid) {
+                    SlotSmem<C>& s = sm.slot[L.slot];
+                    if (s.active) {
+                        if (P.vj) phase_digest_lane<C>(s, L.t, sm.bra.i0, sm.bra.j0, P.n, P.n_dm_j, P.dmj, nullptr, P.vj, nullptr,
+                                                       P.n_dm_j == 1 ? L.jij : nullptr);
+                        if (P.vk) phase_digest_lane<C>(s, L.t, sm.bra.i0, sm.bra.j0, P.n, P.n_dm_k, nullptr, P.dmk, nullptr, P.vk, nullptr);
+                    }
+                }
+            B2_END
+        } else {
+            // one density at a time: the lanes' sums go through the slot's scratch in NRND rounds, and one lane per distinct
+            // K / J[kl] element issues its reduction (DigestCfg)
+            using DG = DigestCfg<C>;
+            const int ndm_j = P.vj ? P.n_dm_j : 0, ndm_k = P.vk ? P.n_dm_k : 0;
+            const size_t n2 = (size_t)P.n * P.n;
+            for (int idm = 0; idm < (ndm_j > ndm_k ? ndm_j : ndm_k); idm++) {
+                const double* Dj = idm < ndm_j ? P.dmj + idm * n2 : nullptr;
+                const double* Dk = idm < ndm_k ? P.dmk + idm * n2 : nullptr;
+                double* J = idm < ndm_j ? P.vj + idm * n2 : nullptr;
+                double* K = idm < ndm_k ? P.vk + idm * n2 : nullptr;
+                B2_GROUP_LANES(lt)
+                    LaneCtx<C>& L = B2_CTX(tid0 + lt);
+                    L.jkl = 0.0;
+                    if (L.valid && Dj) {
+                        const SlotSmem<C>& s = sm.slot[L.slot];
+                        if (s.active) L.jkl = digest_j<C>(s, L.t, sm.bra.i0, sm.bra.j0, P.n, Dj, J, P.n_dm_j == 1 ? L.jij : nullptr);
+                    }
+                B2_END
+                B2_UNROLL
+                for (int rnd = 0; rnd < DG::NRND; rnd++) {
+                    group_sync<C>(grp);   // phase D, or the previous round's flush, is done with H
+                    B2_GROUP_LANES(lt)
+                        LaneCtx<C>& L = B2_CTX(tid0 + lt);
+                        if (L.valid) {
+                            SlotSmem<C>& s = sm.slot[L.slot];
+                            if (s.active) phase_digest<C>(s, L.t, rnd * DG::RPR, sm.bra.i0, sm.bra.j0, P.n, Dk, L.jkl);
+                        }
+                    B2_END
+                    group_sync<C>(grp);
+                    B2_GROUP_LANES(lt)
+                        LaneCtx<C>& L = B2_CTX(tid0 + lt);
+                        if (L.valid) {
+                            const SlotSmem<C>& s = sm.slot[L.slot];
+                            if (s.active) digest_flush<C>(s, L.t.g, rnd * DG::RPR, sm.bra.i0, sm.bra.j0, P.n, J, K);
+                        }
+                    B2_END
                 }
             }
-        B2_END
+        }
         group_sync<C>(grp);
     }
 }

@@ -471,8 +471,165 @@ inline void red_add(double* addr, double val) { *addr += val; }
 #define B2_LDG(p) (*(p))
 #endif
 
+// Every K element and J[kl] of a quartet collects sums from several of its lanes: K[i0+a, kc] from all lanes of the same c,
+// J[kc, ld] from the NP parts, and so on (a (dd|dp) quartet has 648 K sums for 108 distinct K elements).  So the lanes do not
+// reduce their sums into global memory one by one: each lane writes its DigestCfg::NE sums into the slot's scratch (the 2-D
+// integral array H, dead once phase D is done), one row per sum and one column per lane, and then one lane per distinct
+// element adds that element's contributors in lane order and issues ONE reduction.  Where H cannot hold all NE rows of the
+// quartet's G lanes, the rows go through it in NRND rounds of RPR rows.  Rows of a lane (p, c, d):
+//   [0, NI)              kik[a]  -> K[i0+a, kc]            contributors: the lanes of the same c
+//   [NI, 2NI)            kil[a]  -> K[i0+a, ld]            the lanes of the same d
+//   [2NI, 2NI+NJP)       kjk[bb] -> K[j0+p*NJP+bb, kc]     the lanes of the same p and c
+//   [2NI+NJP, 2NI+2NJP)  kjl[bb] -> K[j0+p*NJP+bb, ld]     the lanes of the same p and d
+//   2NI+2NJP             jkl     -> J[kc, ld]              the lanes of the same c and d
 template <class C>
-B2_HD void phase_digest(const SlotSmem<C>& s, const ThreadCtx<C>& t, int i0, int j0, int n, int n_dm,
+struct DigestCfg {
+    static constexpr int NE = 2 * C::NI + 2 * C::NJP + 1;
+    static constexpr int RPR = C::PB * 3 * C::NR * C::HSP / C::G;   // rows per round
+    static constexpr int NRND = RPR > 0 ? (NE + RPR - 1) / RPR : 1;
+    // row family f (the five lines above): its first row, and the distinct elements each of its rows feeds
+    static B2_HD constexpr int row0(int f)
+    {
+        return f == 0 ? 0 : f == 1 ? C::NI : f == 2 ? 2 * C::NI : f == 3 ? 2 * C::NI + C::NJP : f == 4 ? 2 * C::NI + 2 * C::NJP : NE;
+    }
+    static B2_HD constexpr int nel(int f)
+    {
+        return f == 0 ? C::NK : f == 1 ? C::NL : f == 2 ? C::NP * C::NK : f == 3 ? C::NP * C::NL : C::NKL;
+    }
+};
+
+// The J part of lane (p, c, d) for one density D: returns jkl = sum_ab v D[ij] (its row of the scratch) and adds the
+// J[ij] of the bra block, which has one contributor per lane and element, to jacc (the stationary bra pair's registers,
+// flushed once per CTA) or, without jacc, straight to J.  It runs before the rounds (phase_digest) in a phase of its own,
+// so that its density loads are not scheduled next to theirs.
+template <class C>
+B2_HD double digest_j(const SlotSmem<C>& s, const ThreadCtx<C>& t, int i0, int j0, int n, const double* D, double* J,
+                      double* jacc)
+{
+    const double dkl = 2.0 * s.fac * B2_LDG(&D[(size_t)(s.k0 + t.c) * n + s.l0 + t.d]);
+    const int jb0 = j0 + t.p * C::NJP;
+    double jkl = 0.0;
+    B2_UNROLL
+    for (int bb = 0; bb < C::NJP; bb++) {
+        B2_UNROLL
+        for (int a = 0; a < C::NI; a++) {
+            const double val = t.v[bb * C::NI + a];
+            const size_t ij = (size_t)(i0 + a) * n + (jb0 + bb);
+            jkl += val * B2_LDG(&D[ij]);
+            if (jacc) jacc[bb * C::NI + a] += val * dkl;
+            else red_add(&J[ij], val * dkl);
+        }
+    }
+    return jkl;
+}
+
+// Lane (p, c, d)'s sums of rows [r0, r0 + RPR), written to the slot's scratch: row r at H + (r - r0) * G + g.  The K sums
+// are computed in the round that stores them, so the register block is the only state a lane carries from round to round.
+// Dk: this density (null: no K of it, those rows are zero); jkl: the J row (digest_j, zero without J).
+template <class C>
+B2_HD void phase_digest(SlotSmem<C>& s, const ThreadCtx<C>& t, int r0, int i0, int j0, int n, const double* Dk, double jkl)
+{
+    using DG = DigestCfg<C>;
+    static_assert(DG::RPR >= 1, "the 2-D integral array of a slot must hold one row of the quartet's lanes");
+    const int r1 = r0 + DG::RPR;
+    const int kc = s.k0 + t.c, ld = s.l0 + t.d;
+    const int jb0 = j0 + t.p * C::NJP;
+    double* X = &s.H[0][0][0][0] + t.g;
+    if (!Dk) {
+        B2_UNROLL
+        for (int r = 0; r < DG::NE; r++)
+            if (r >= r0 && r < r1) X[(r - r0) * C::G] = r == DG::NE - 1 ? jkl : 0.0;
+        return;
+    }
+    // the density columns the rows of this round read: D[jb, ld] (kik), D[jb, kc] (kil), D[i0+a, ld] (kjk), D[i0+a, kc] (kjl)
+    const auto in_round = [&](int f_) { return DG::row0(f_) < r1 && DG::row0(f_ + 1) > r0; };
+    double djl[C::NJP], djk[C::NJP], dil[C::NI], dik[C::NI];
+    B2_UNROLL
+    for (int bb = 0; bb < C::NJP; bb++) {
+        if (in_round(0)) djl[bb] = B2_LDG(&Dk[(size_t)(jb0 + bb) * n + ld]);
+        if (in_round(1)) djk[bb] = B2_LDG(&Dk[(size_t)(jb0 + bb) * n + kc]);
+    }
+    B2_UNROLL
+    for (int a = 0; a < C::NI; a++) {
+        if (in_round(2)) dil[a] = B2_LDG(&Dk[(size_t)(i0 + a) * n + ld]);
+        if (in_round(3)) dik[a] = B2_LDG(&Dk[(size_t)(i0 + a) * n + kc]);
+    }
+    B2_UNROLL
+    for (int r = 0; r < DG::NE; r++) {
+        if (r < r0 || r >= r1) continue;
+        double sum = 0.0;
+        if (r < 2 * C::NI) {                      // kik[a] = sum_b v D[jb, ld],  kil[a] = sum_b v D[jb, kc]
+            const int a = r < C::NI ? r : r - C::NI;
+            B2_UNROLL
+            for (int bb = 0; bb < C::NJP; bb++) sum += t.v[bb * C::NI + a] * (r < C::NI ? djl[bb] : djk[bb]);
+        } else if (r < 2 * C::NI + 2 * C::NJP) {  // kjk[b] = sum_a v D[i0+a, ld],  kjl[b] = sum_a v D[i0+a, kc]
+            const int bb = r < 2 * C::NI + C::NJP ? r - 2 * C::NI : r - 2 * C::NI - C::NJP;
+            B2_UNROLL
+            for (int a = 0; a < C::NI; a++) sum += t.v[bb * C::NI + a] * (r < 2 * C::NI + C::NJP ? dil[a] : dik[a]);
+        } else {
+            sum = jkl;
+        }
+        X[(r - r0) * C::G] = sum;
+    }
+}
+
+// the distinct elements fed by rows [r0, r0 + RPR), tasks g, g + G, ... of the quartet: each sums its contributors in lane
+// order and issues one reduction.  J / K: the outputs of this density (null: not computed).
+template <class C>
+B2_HD void digest_flush(const SlotSmem<C>& s, int g, int r0, int i0, int j0, int n, double* J, double* K)
+{
+    using DG = DigestCfg<C>;
+    const int r1 = r0 + DG::RPR < DG::NE ? r0 + DG::RPR : DG::NE;
+    const double* X = &s.H[0][0][0][0];
+    const double f = s.fac;
+    const int k0 = s.k0, l0 = s.l0;
+    B2_UNROLL
+    for (int fam = 0; fam < 5; fam++) {
+        const int lo = DG::row0(fam) > r0 ? DG::row0(fam) : r0;
+        const int hi = DG::row0(fam + 1) < r1 ? DG::row0(fam + 1) : r1;
+        if (hi <= lo || (fam < 4 ? K : J) == nullptr) continue;
+        const int nel = DG::nel(fam);
+        for (int task = g; task < (hi - lo) * nel; task += C::G) {
+            const int row = lo + task / nel, el = task - (task / nel) * nel;
+            const double* x = X + (row - r0) * C::G;
+            double sum = 0.0;
+            if (fam == 0) {          // K[i0+a, kc], c = el: lanes p*NKL + d*NK + c
+                B2_UNROLL
+                for (int p = 0; p < C::NP; p++) {
+                    B2_UNROLL
+                    for (int d = 0; d < C::NL; d++) sum += x[p * C::NKL + d * C::NK + el];
+                }
+                red_add(&K[(size_t)(i0 + row) * n + k0 + el], f * sum);
+            } else if (fam == 1) {   // K[i0+a, ld], d = el
+                B2_UNROLL
+                for (int p = 0; p < C::NP; p++) {
+                    B2_UNROLL
+                    for (int c = 0; c < C::NK; c++) sum += x[p * C::NKL + el * C::NK + c];
+                }
+                red_add(&K[(size_t)(i0 + row - C::NI) * n + l0 + el], f * sum);
+            } else if (fam == 2) {   // K[j0+p*NJP+bb, kc], el = p*NK + c
+                const int p = el / C::NK, c = el - p * C::NK;
+                B2_UNROLL
+                for (int d = 0; d < C::NL; d++) sum += x[p * C::NKL + d * C::NK + c];
+                red_add(&K[(size_t)(j0 + p * C::NJP + row - 2 * C::NI) * n + k0 + c], f * sum);
+            } else if (fam == 3) {   // K[j0+p*NJP+bb, ld], el = p*NL + d
+                const int p = el / C::NL, d = el - p * C::NL;
+                B2_UNROLL
+                for (int c = 0; c < C::NK; c++) sum += x[p * C::NKL + d * C::NK + c];
+                red_add(&K[(size_t)(j0 + p * C::NJP + row - 2 * C::NI - C::NJP) * n + l0 + d], f * sum);
+            } else {                 // J[kc, ld], el = d*NK + c
+                B2_UNROLL
+                for (int p = 0; p < C::NP; p++) sum += x[p * C::NKL + el];
+                red_add(&J[(size_t)(k0 + el % C::NK) * n + l0 + el / C::NK], 2.0 * f * sum);
+            }
+        }
+    }
+}
+
+// Phase E without the scratch: every lane reduces its own sums straight into J and K (the classes of
+// class_reduces_per_lane).
+template <class C>
+B2_HD void phase_digest_lane(const SlotSmem<C>& s, const ThreadCtx<C>& t, int i0, int j0, int n, int n_dm,
                         const double* dmj, const double* dmk, double* vj, double* vk, double* jacc)
 {
     const double f = s.fac;
